@@ -32,7 +32,7 @@ class IgemmDesc(C.Structure):
         ("bias", C.c_void_p), ("bias2", C.c_void_p), ("rows_per_bias2", C.c_int), ("ld_bias2", C.c_long),
         ("residual", C.c_void_p), ("ld_res", C.c_long),
         ("out_scale", C.c_float), ("act", C.c_int), ("flags", C.c_int), ("block_n", C.c_int), ("max_ctas", C.c_int),
-        ("debug_cycles", C.c_void_p), ("colstats", C.c_void_p),
+        ("colstats", C.c_void_p),
     ]
 
 

@@ -1,4 +1,4 @@
-"""B200 mirror of diffusers' `AutoencoderKL` (SD VAE) as the reference uses it:
+"""Mirror of diffusers' `AutoencoderKL` (SD VAE) as the reference uses it:
   encode: utils/common.py:12-20 (`vae.encode(t).latent_dist.mode()`), train.py:747
   decode: models/pipeline.py:200 -> TextToVideoSDPipeline.decode_latents -> `vae.decode(latents).sample`
   surface: `.config.scaling_factor`, `.config.block_out_channels`, `.config.force_upcast`, `.enable_slicing()`,
@@ -6,7 +6,7 @@
 Same sub-module names as diffusers 0.24 (`encoder.down_blocks.i.resnets.j`, `mid_block.attentions.0.to_q`, ...), legacy
 `query/key/value/proj_attn` checkpoint keys are converted on load.
 
-All convolutions (3x3, stride-2, 1x1) run on the tcgen05 implicit-GEMM kernel over channels-last frames; GroupNorm+SiLU on
+All convolutions (3x3, stride-2, 1x1) run on the wgmma implicit-GEMM kernel over channels-last frames; GroupNorm+SiLU on
 the fused norm kernels; the single-head (d=512) mid-block attention as two batched implicit GEMMs around a row softmax.
 Frames are independent -> processed in chunks (`frame_chunk`) to bound the 128ch x 512^2 activations; `enable_slicing()`
 is accepted and does not change results.
@@ -159,7 +159,7 @@ class AutoencoderKL(ModelBase):
         if prep is not None and prep.dtype == p0.dtype and prep.device == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16) or not p0.is_cuda:
-            raise TypeError("AutoencoderKL must be fp16/bf16 on a CUDA device for the sm_100a path (no fallback)")
+            raise TypeError("AutoencoderKL must be fp16/bf16 on a CUDA device for the sm_90a path (no fallback)")
         prep = self._build_prepared(p0.dtype, p0.device)
         self.__dict__["_aab_prepared"] = prep
         return prep

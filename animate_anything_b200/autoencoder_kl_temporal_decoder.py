@@ -1,4 +1,4 @@
-"""B200 mirror of diffusers' `AutoencoderKLTemporalDecoder` (the SVD VAE) as the reference uses it:
+"""Mirror of diffusers' `AutoencoderKLTemporalDecoder` (the SVD VAE) as the reference uses it:
 `MaskStableVideoDiffusionPipeline.__call__` encodes the conditioning image (`_encode_vae_image`, models/pipeline.py:359-362)
 and decodes the final latents in chunks of `decode_chunk_size` frames (`decode_latents`, :456).
 

@@ -1,4 +1,4 @@
-"""B200 mirror of `transformers.CLIPTextModel` as the reference uses it: `LatentToVideoPipeline._encode_prompt`
+"""Mirror of `transformers.CLIPTextModel` as the reference uses it: `LatentToVideoPipeline._encode_prompt`
 (models/pipeline.py:136 -> diffusers TextToVideoSDPipeline._encode_prompt) calls
 `self.text_encoder(text_input_ids.to(device), attention_mask=None)[0]` on the model loaded at train.py:88
 (`CLIPTextModel.from_pretrained(path, subfolder="text_encoder")`), cast to fp16 on the GPU at train.py:851.
@@ -9,7 +9,7 @@ same call signature and outputs (`[0]` = last_hidden_state [B, L, C], `.pooler_o
 
 Execution (all through the C-ABI, no library GEMM / SDPA):
   token + position embedding   -> `aab_embed_tokens`
-  per layer: LayerNorm -> fused q|k|v Linear (one [3C, C] tcgen05 GEMM, bias in the epilogue) -> causal head-dim-64 flash
+  per layer: LayerNorm -> fused q|k|v Linear (one [3C, C] wgmma GEMM, bias in the epilogue) -> causal head-dim-64 flash
              attention (`aab_flash_attn_d64`, causal bit) -> out_proj (+ residual in the epilogue) -> LayerNorm ->
              fc1 (+ GELU / quick-GELU) -> fc2 (+ residual)
   final LayerNorm; pooled row gathered with `aab_copy2d`.
@@ -94,7 +94,7 @@ class CLIPTextModel(ModelBase):
             eos_token_id=eos_token_id, projection_dim=projection_dim, pad_token_id=pad_token_id,
             bos_token_id=bos_token_id))
         if hidden_size != 64 * num_attention_heads:
-            raise ValueError("the sm_100a attention kernel is specialised for head_dim 64 (ViT-H/14 and ViT-L/14 text towers)")
+            raise ValueError("the sm_90a attention kernel is specialised for head_dim 64 (ViT-H/14 and ViT-L/14 text towers)")
         if hidden_act not in ("gelu", "quick_gelu"):
             raise ValueError(f"hidden_act {hidden_act!r} is not a CLIP text activation")
         if max_position_embeddings > 128:
@@ -132,7 +132,7 @@ class CLIPTextModel(ModelBase):
         if prep is not None and prep["dtype"] == p0.dtype and prep["device"] == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16) or not p0.is_cuda:
-            raise TypeError("CLIPTextModel must be fp16/bf16 on a CUDA device for the sm_100a path (train.py:851 casts "
+            raise TypeError("CLIPTextModel must be fp16/bf16 on a CUDA device for the sm_90a path (train.py:851 casts "
                             "it to half on cuda); there is no library / CPU fallback")
         dt = p0.dtype
         f32 = lambda t: t.detach().float().contiguous()

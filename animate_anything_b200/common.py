@@ -1,7 +1,7 @@
 """Mirror of the reference's `utils/common.py` functions that sit on the inference path (SURVEY 8a rows a20, a22):
 what `train.py:745-757` (eval) and `app.py:80` call between loading the prompt image and `pipeline.__call__`.
 
-Same names, argument order and return values as the reference; the arithmetic runs in the sm_100a kernels
+Same names, argument order and return values as the reference; the arithmetic runs in the sm_90a kernels
 (`aab_vae_enc_finalize`, `aab_add_noise`), the random numbers come from `torch.randn` exactly as in the reference
 (utils/common.py:44 / :27), so a seeded run draws the same noise.
 """

@@ -3,11 +3,11 @@
 // 1. aab_flash_attn_d64 — spatial self-attention and text cross-attention of diffusers' BasicTransformerBlock
 //    (head_dim 64; reference call sites: Transformer2DModel built at models/unet_3d_blocks.py:287-296,446-456,
 //    681-691, processor AttnProcessor2_0 -> F.scaled_dot_product_attention installed by train.py:124-138).
-//    Flash-style: one CTA owns 256 query rows (two 128-row tiles, ping-pong) of one (batch, head);
-//    S = Q.K^T and O_j = P_j.V_j run on tcgen05 with S / O_j in TMEM; two softmax warpgroups do the online
-//    softmax (exp2, fp32 running max / sum), write P (16-bit) into 128B-swizzled shared memory as the A operand of
-//    the second MMA and accumulate O in registers.  K/V tiles are TMA-loaded into a 3-stage ring shared by both
-//    query tiles.  Keys past Lk (e.g. 77 text tokens in a 128-key tile) are masked to -inf.
+//    Flash-style on the Hopper warpgroup MMA: one CTA owns 128 query rows of one (batch, head), split between two
+//    consumer warpgroups of 64 rows.  S = Q.K^T (wgmma, both operands in shared memory) lands in registers, the online
+//    softmax (exp2, fp32 running max / sum) runs on those registers, and P is fed back as the register A operand of
+//    O += P.V (wgmma, V MN-major in shared memory).  64-key K/V blocks are TMA-loaded into a 3-stage ring by a producer
+//    warp.  Keys past Lk (e.g. 77 text tokens) are masked to -inf.
 //
 // 2. aab_temporal_attn_d64 — self-attention over the frame axis (T <= 32) of TransformerTemporalModel
 //    (models/unet_3d_blocks.py:299-306,459-467,694-701; called without encoder_hidden_states so both attn1 and attn2
@@ -16,59 +16,22 @@
 //    FLOPs: CUDA cores, one warp per (position, head).
 #include "common.cuh"
 #include "igemm.h"
+#include "wgmma.cuh"
 #include <stdlib.h>
 
 namespace aab {
 
-constexpr int FA_THREADS = 320;       // warp0 TMA, warp1 MMA, warps 2-5 softmax tile A, warps 6-9 softmax tile B
+constexpr int FA_THREADS = 288;       // warpgroups 0, 1: 64 query rows each; warp 8: TMA producer
+constexpr int FA_BKV = 64;            // keys per K/V block
 constexpr int FA_KV_STAGES = 3;
-constexpr int FA_TILE_BYTES = 128 * 64 * 2;   // 16 KiB: one [128 x 64] 16-bit tile
-constexpr int FA_SMEM_BYTES = 2 * FA_TILE_BYTES               /* Q A,B */
-                              + FA_KV_STAGES * 2 * FA_TILE_BYTES /* K,V ring */
-                              + 2 * 2 * FA_TILE_BYTES          /* P A,B: two 64-key halves each */
-                              + 1024 + 256;
+constexpr int FA_Q_BYTES = 128 * 64 * 2;       // 16 KiB: [128 x 64] 16-bit
+constexpr int FA_KV_BYTES = FA_BKV * 64 * 2;   // 8 KiB: [64 x 64] 16-bit
+constexpr int FA_SMEM_BYTES = FA_Q_BYTES + FA_KV_STAGES * 2 * FA_KV_BYTES + 1024 + 256;
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// packed fp32 pairs (Blackwell FFMA2 / FADD2): half the issue slots of the softmax's scale-and-subtract, row-sum and O updates
-__device__ __forceinline__ float2 ffma2(float ax, float ay, float2 b, float2 c) {
-  float2 d;
-  asm("{\n.reg .b64 ra, rb, rc, rd;\nmov.b64 ra, {%2, %3};\nmov.b64 rb, {%4, %5};\nmov.b64 rc, {%6, %7};\n"
-      "fma.rn.f32x2 rd, ra, rb, rc;\nmov.b64 {%0, %1}, rd;\n}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(ax), "f"(ay), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  float2 d;
-  asm("{\n.reg .b64 ra, rb, rd;\nmov.b64 ra, {%2, %3};\nmov.b64 rb, {%4, %5};\nadd.rn.f32x2 rd, ra, rb;\nmov.b64 {%0, %1}, rd;\n}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-
-// 2^t for a pair of t <= 0 on the FMA / ALU pipes instead of the MUFU (16 results / clk / SM, the busiest pipe of the d=64 softmax:
-// ncu 56 % of peak in round 2a): t = j + f, j = round(t) through the 1.5 * 2^23 magic add, f in [-0.5, 0.5], 2^f by a degree-4
-// polynomial (max relative error 2.7e-6, far below the 16-bit rounding of P), 2^j by an integer add into the exponent field.
-__device__ __forceinline__ float2 exp2_poly2(float2 t) {
-  t.x = fmaxf(t.x, -126.f);
-  t.y = fmaxf(t.y, -126.f);
-  const float2 magic = make_float2(12582912.f, 12582912.f);
-  const float2 tt = fadd2(t, magic);
-  const float2 r = fadd2(tt, make_float2(-12582912.f, -12582912.f));
-  const float2 f = ffma2(r.x, r.y, make_float2(-1.f, -1.f), t);
-  float2 q = ffma2(f.x, f.y, make_float2(0.00956052f, 0.00956052f), make_float2(0.05591708f, 0.05591708f));
-  q = ffma2(q.x, q.y, f, make_float2(0.24024981f, 0.24024981f));
-  q = ffma2(q.x, q.y, f, make_float2(0.69312196f, 0.69312196f));
-  q = ffma2(q.x, q.y, f, make_float2(0.99999919f, 0.99999919f));
-  float2 o;
-  o.x = __int_as_float(__float_as_int(q.x) + (__float_as_int(tt.x) << 23));
-  o.y = __int_as_float(__float_as_int(q.y) + (__float_as_int(tt.y) << 23));
-  return o;
 }
 
 struct FaParams {
@@ -79,588 +42,161 @@ struct FaParams {
   long out_batch_stride;   // elements between consecutive batches of the output
   int out_col0;
   float scale_log2;
-  int is_bf16;
   int causal;              // key j visible to query i iff j <= i (CLIP text tower); host guarantees Lq == Lk <= 128
 };
 
-__global__ void __launch_bounds__(FA_THREADS, 1)
+// Fragment layout of an m64nN fp32 accumulator (and of the register A operand): thread `lane` of warp `wq` in the warpgroup
+// holds, for i in [0, N/2), row 16 wq + lane / 4 + 8 ((i >> 1) & 1) and column 8 (i >> 2) + 2 (lane & 3) + (i & 1).
+template <bool BF16>
+__global__ void __launch_bounds__(FA_THREADS, 2)
 flash_attn_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const FaParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smQ = smem;                                    // [2][16K]
-  uint8_t* smK = smQ + 2 * FA_TILE_BYTES;                 // [ST][16K]
-  uint8_t* smV = smK + FA_KV_STAGES * FA_TILE_BYTES;      // [ST][16K]
-  uint8_t* smP = smV + FA_KV_STAGES * FA_TILE_BYTES;      // [2 tiles][2 halves][16K]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smP + 4 * FA_TILE_BYTES);
-  uint64_t* q_full = bars;                 // 1
-  uint64_t* kv_full = bars + 1;            // ST
-  uint64_t* kv_empty = kv_full + FA_KV_STAGES;
-  uint64_t* s_full = kv_empty + FA_KV_STAGES;   // 2
-  uint64_t* p_ready = s_full + 2;               // 2
-  uint64_t* o_full = p_ready + 2;               // 2
-  uint64_t* o_free = o_full + 2;                // 2
-  uint64_t* p_free = o_free + 2;                // 2: P.V of the previous block has consumed the P tile
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(p_free + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int q0 = blockIdx.x * 256;
-  const int head = blockIdx.y;
-  const int b = blockIdx.z;
-  const int bkv = b / p.kv_batch_div;
-  const int nkv = (p.Lk + 127) / 128;
-  const bool bf16 = p.is_bf16 != 0;
-
-  if (warp == 0 && elect_one()) {
-    prefetch_tmap(&tmQ);
-    prefetch_tmap(&tmK);
-    prefetch_tmap(&tmV);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      mbar_init(q_full, 1);
-      for (int i = 0; i < FA_KV_STAGES; ++i) {
-        mbar_init(&kv_full[i], 1);
-        mbar_init(&kv_empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&p_ready[i], 128);
-        mbar_init(&o_full[i], 1);
-        mbar_init(&o_free[i], 128);
-        mbar_init(&p_free[i], 1);
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  // TMEM columns: S_A [0,128) S_B [128,256) O_A [256,320) O_B [320,384)
-
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, 2 * FA_TILE_BYTES);
-      tma_load_3d(smQ, &tmQ, q_full, p.q_col0 + head * 64, q0, b);
-      tma_load_3d(smQ + FA_TILE_BYTES, &tmQ, q_full, p.q_col0 + head * 64, q0 + 128, b);
-      for (int j = 0; j < nkv; ++j) {
-        const int s = j % FA_KV_STAGES;
-        const uint32_t ph = (j / FA_KV_STAGES) & 1;
-        mbar_wait(&kv_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&kv_full[s], 2 * FA_TILE_BYTES);
-        tma_load_3d(smK + s * FA_TILE_BYTES, &tmK, &kv_full[s], p.k_col0 + head * 64, j * 128, bkv);
-        tma_load_3d(smV + s * FA_TILE_BYTES, &tmV, &kv_full[s], p.v_col0 + head * 64, j * 128, bkv);
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc_s = make_idesc_f16(bf16 ? 1 : 0, 128, 128, 0, 0);
-    const uint32_t idesc_o = make_idesc_f16(bf16 ? 1 : 0, 128, 64, 0, 1);   // B (=V) is MN-major
-    auto issue_s = [&](int tile, int s) {
-      if (elect_one()) {
-        const uint32_t qa = smem_u32(smQ + tile * FA_TILE_BYTES);
-        const uint32_t ka = smem_u32(smK + s * FA_TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_f16_ss(tmem_base + tile * 128, make_desc_kmajor_sw128(qa + k * 32), make_desc_kmajor_sw128(ka + k * 32),
-                      idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[tile]);
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [&](int tile, int s) {
-      if (elect_one()) {
-        const uint32_t pa = smem_u32(smP + tile * 2 * FA_TILE_BYTES);
-        const uint32_t va = smem_u32(smV + s * FA_TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_f16_ss(tmem_base + 256 + tile * 64,
-                      make_desc_kmajor_sw128(pa + (k >> 2) * FA_TILE_BYTES + (k & 3) * 32),
-                      make_desc_mnmajor_sw128(va + k * 2048, 8192), idesc_o, k > 0 ? 1u : 0u);
-        umma_commit(&o_full[tile]);
-        umma_commit(&p_free[tile]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    mbar_wait(&kv_full[0], 0);
-    tc_fence_after();
-    // (An in-phase order -- both tiles' MMAs interleaved instruction by instruction so that consecutive tcgen05.mma never share
-    // an accumulator, S(j+1) issued as soon as both warpgroups had loaded S(j) -- was built and measured: 1538 us against 1234
-    // for L = 4096.  The staggered order below lets one warpgroup's softmax overlap the other's MMAs, and the softmax, not the
-    // tensor pipe (28 % busy), is what this kernel waits for: profiles/r02_flash_softmax.md.)
-    issue_s(0, 0);
-    issue_s(1, 0);
-    for (int j = 0; j < nkv; ++j) {
-      const int s = j % FA_KV_STAGES;
-      const uint32_t jph = j & 1;
-      const int sn = (j + 1) % FA_KV_STAGES;
-      const uint32_t phn = ((j + 1) / FA_KV_STAGES) & 1;
-#pragma unroll
-      for (int tile = 0; tile < 2; ++tile) {
-        // softmax(j) of this tile is done: first give it S(j+1) (so that it never waits for a score tile), then run
-        // P.V(j) once the (deferred) read-back of O(j-1) has released the O columns
-        mbar_wait(&p_ready[tile], jph);
-        if (j + 1 < nkv) {
-          if (tile == 0) mbar_wait(&kv_full[sn], phn);
-          tc_fence_after();
-          issue_s(tile, sn);
-        }
-        if (j > 0) mbar_wait(&o_free[tile], jph ^ 1);
-        tc_fence_after();
-        issue_pv(tile, s);
-        if (tile == 1 && elect_one()) umma_commit(&kv_empty[s]);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ------------------------------------------------------------ softmax warpgroups
-    const int tile = (warp - 2) >> 2;               // 0: rows q0..q0+127, 1: q0+128..
-    const int qd = warp & 3;                        // TMEM lane quarter
-    const int row = qd * 32 + lane_id();
-    const uint32_t t_s = tmem_base + tile * 128 + (static_cast<uint32_t>(qd * 32) << 16);
-    const uint32_t t_o = tmem_base + 256 + tile * 64 + (static_cast<uint32_t>(qd * 32) << 16);
-    uint8_t* prow = smP + tile * 2 * FA_TILE_BYTES + row * 128;
-    float o_acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) o_acc[i] = 0.f;
-    float m_run = -INFINITY;
-    float l_run = 0.f;
-    float alpha_prev = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const uint32_t jph = j & 1;
-      mbar_wait(&s_full[tile], jph);
-      tc_fence_after();
-      const int kbase = j * 128;
-      int valid = p.Lk - kbase;                     // keys of this block that exist (>= 128: no masking needed)
-      if (p.causal) {                               // per-row limit: keys kbase .. min(Lk, q) (one block: Lk <= 128)
-        const int vis = q0 + tile * 128 + row - kbase + 1;
-        valid = vis < valid ? vis : valid;
-      }
-      float alpha, lsum = 0.f;
-      if (valid >= 128 && !p.causal) {
-        // ---------------- common case (no per-element predicates).  Round 2b: four independent partial maxima / packed partial sums
-        // (the round-1 loops were one dependent chain each), packed fp32 scale-and-subtract; (a) the tcgen05.ld of chunk c + 1 is in flight
-        // while chunk c is processed (two 32-register buffers), the exponential pass walks the chunks 3, 0, 1, 2 so that the last
-        // chunk of the max pass is reused without a reload; (b) one pair in four of the exponentials is evaluated by
-        // exp2_poly2 on the FMA pipes.
-        uint32_t ra[32], rb[32];
-        float mxa = -INFINITY, mxb = -INFINITY, mxc = -INFINITY, mxd = -INFINITY;
-        auto max32 = [&](const uint32_t* r) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            mxa = fmaxf(mxa, fmaxf(__uint_as_float(r[i]), __uint_as_float(r[i + 1])));
-            mxb = fmaxf(mxb, fmaxf(__uint_as_float(r[i + 2]), __uint_as_float(r[i + 3])));
-            mxc = fmaxf(mxc, fmaxf(__uint_as_float(r[i + 4]), __uint_as_float(r[i + 5])));
-            mxd = fmaxf(mxd, fmaxf(__uint_as_float(r[i + 6]), __uint_as_float(r[i + 7])));
-          }
-        };
-        tmem_ld_32x32(t_s, ra);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s + 32, rb);
-        max32(ra);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s + 64, ra);
-        max32(rb);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s + 96, rb);
-        max32(ra);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s, ra);            // chunk 0 again, for the exponential pass (chunk 3 stays in rb)
-        max32(rb);
-        const float mx = fmaxf(fmaxf(mxa, mxb), fmaxf(mxc, mxd));
-        const float m_new = fmaxf(m_run, mx * p.scale_log2);
-        alpha = fast_exp2(m_run - m_new);
-        m_run = m_new;
-        if (j > 0) mbar_wait(&p_free[tile], jph ^ 1);   // P.V(j-1) has read the P tile
-        const float2 sc2 = make_float2(p.scale_log2, p.scale_log2);
-        const float2 nm2 = make_float2(-m_new, -m_new);
-        float2 ls[4] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        auto exp32 = [&](const uint32_t* r, int c) {
-          uint8_t* hp = prow + (c >> 1) * FA_TILE_BYTES;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float2 e[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 t = ffma2(__uint_as_float(r[g * 8 + 2 * i]), __uint_as_float(r[g * 8 + 2 * i + 1]), sc2, nm2);
-              e[i] = (i == 3) ? exp2_poly2(t) : make_float2(fast_exp2(t.x), fast_exp2(t.y));
-              ls[i] = fadd2(ls[i], e[i]);
-            }
-            uint4 u;
-            u.x = pack2(e[0].x, e[0].y, bf16);
-            u.y = pack2(e[1].x, e[1].y, bf16);
-            u.z = pack2(e[2].x, e[2].y, bf16);
-            u.w = pack2(e[3].x, e[3].y, bf16);
-            const int chunk = (c & 1) * 4 + g;
-            *reinterpret_cast<uint4*>(hp + ((chunk ^ (row & 7)) << 4)) = u;
-          }
-        };
-        exp32(rb, 3);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s + 32, rb);
-        exp32(ra, 0);
-        tmem_ld_wait();
-        tmem_ld_32x32(t_s + 64, ra);
-        exp32(rb, 1);
-        tmem_ld_wait();
-        exp32(ra, 2);
-        const float2 l01 = fadd2(ls[0], ls[1]), l23 = fadd2(ls[2], ls[3]);
-        lsum = (l01.x + l01.y) + (l23.x + l23.y);
-      } else {
-        // ---------------- tail block: keys >= valid are masked to -inf / 0
-        float mx = -INFINITY;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32(t_s + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c * 32 + i < valid) mx = fmaxf(mx, __uint_as_float(r[i]));
-        }
-        const float m_new = fmaxf(m_run, mx * p.scale_log2);
-        alpha = fast_exp2(m_run - m_new);
-        m_run = m_new;
-        if (j > 0) mbar_wait(&p_free[tile], jph ^ 1);
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32(t_s + c * 32, r);
-          tmem_ld_wait();
-          uint8_t* hp = prow + (c >> 1) * FA_TILE_BYTES;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float e[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float x = fast_exp2(fmaf(__uint_as_float(r[g * 8 + i]), p.scale_log2, -m_new));
-              e[i] = (c * 32 + g * 8 + i < valid) ? x : 0.f;
-              lsum += e[i];
-            }
-            uint4 u;
-            u.x = pack2(e[0], e[1], bf16);
-            u.y = pack2(e[2], e[3], bf16);
-            u.z = pack2(e[4], e[5], bf16);
-            u.w = pack2(e[6], e[7], bf16);
-            const int chunk = (c & 1) * 4 + g;
-            *reinterpret_cast<uint4*>(hp + ((chunk ^ (row & 7)) << 4)) = u;
-          }
-        }
-      }
-      l_run = l_run * alpha + lsum;
-      tc_fence_before();
-      fence_proxy_async_smem();
-      mbar_arrive(&p_ready[tile]);
-      // deferred read-back of the previous block: o_acc = alpha_{j-1} * o_acc + O_{j-1}
-      if (j > 0) {
-        mbar_wait(&o_full[tile], jph ^ 1);
-        tc_fence_after();
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32(t_o + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float2 t = ffma2(o_acc[c * 32 + i], o_acc[c * 32 + i + 1], make_float2(alpha_prev, alpha_prev),
-                                   make_float2(__uint_as_float(r[i]), __uint_as_float(r[i + 1])));
-            o_acc[c * 32 + i] = t.x;
-            o_acc[c * 32 + i + 1] = t.y;
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(&o_free[tile]);
-      }
-      alpha_prev = alpha;
-    }
-    {
-      mbar_wait(&o_full[tile], (nkv - 1) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_o + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o_acc[c * 32 + i] = fmaf(o_acc[c * 32 + i], alpha_prev, __uint_as_float(r[i]));
-      }
-    }
-    const int q = q0 + tile * 128 + row;
-    if (q < p.Lq) {
-      const float inv = 1.0f / l_run;
-      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) +
-                                           (static_cast<long>(b) * p.out_batch_stride + static_cast<long>(q) * p.ld_out +
-                                            p.out_col0 + head * 64) * 2);
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        uint4 u;
-        u.x = pack2(o_acc[g * 8 + 0] * inv, o_acc[g * 8 + 1] * inv, bf16);
-        u.y = pack2(o_acc[g * 8 + 2] * inv, o_acc[g * 8 + 3] * inv, bf16);
-        u.z = pack2(o_acc[g * 8 + 4] * inv, o_acc[g * 8 + 5] * inv, bf16);
-        u.w = pack2(o_acc[g * 8 + 6] * inv, o_acc[g * 8 + 7] * inv, bf16);
-        op[g] = u;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ flash v2
-// One 128-query tile per CTA, S DOUBLE-BUFFERED in TMEM: the tensor core computes S(j+1) while the single softmax
-// warpgroup (4 warps, one per SM sub-partition) works on S(j), so the exp2 (MUFU) pipe — the real bound of d=64
-// attention on Blackwell — never waits for an MMA.  The O_j = P_j.V_j read-back is deferred by one block.
-//   TMEM columns: S0 [0,128)  S1 [128,256)  O_j [256,320)
-// SHORT = true (round 2): the key/value sequence fits ONE 128-key block (text cross-attention: 77 tokens).  One K/V stage,
-// 256 TMEM columns (S at 0, O at 128) and 80 KiB of shared memory let two or three CTAs share an SM, so the prologue /
-// load / softmax latencies of one CTA overlap the others' -- v1 (one 192 KiB CTA per SM) spent 160 us on 54 us of work.
-constexpr int FA2_THREADS = 192;      // warp0 TMA, warp1 MMA, warps 2-5 softmax
-constexpr int FA2_SMEM_BYTES = FA_TILE_BYTES + FA_KV_STAGES * 2 * FA_TILE_BYTES + 2 * FA_TILE_BYTES + 1024 + 256;
-constexpr int FA2S_SMEM_BYTES = FA_TILE_BYTES + 1 * 2 * FA_TILE_BYTES + 2 * FA_TILE_BYTES + 1024 + 256;
-
-template <bool SHORT>
-__global__ void __launch_bounds__(FA2_THREADS, SHORT ? 2 : 1)
-flash_attn_d64_v2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                         const __grid_constant__ CUtensorMap tmV, const FaParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int KVS = SHORT ? 1 : FA_KV_STAGES;
-  constexpr uint32_t TCOLS = SHORT ? 256 : 512;
-  constexpr uint32_t O_COL = SHORT ? 128 : 256;
   uint8_t* smQ = smem;
-  uint8_t* smK = smQ + FA_TILE_BYTES;
-  uint8_t* smV = smK + KVS * FA_TILE_BYTES;
-  uint8_t* smP = smV + KVS * FA_TILE_BYTES;      // two 64-key halves
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smP + 2 * FA_TILE_BYTES);
+  uint8_t* smK = smQ + FA_Q_BYTES;                        // [ST][8K]
+  uint8_t* smV = smK + FA_KV_STAGES * FA_KV_BYTES;        // [ST][8K]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smV + FA_KV_STAGES * FA_KV_BYTES);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;
-  uint64_t* kv_empty = kv_full + KVS;
-  uint64_t* s_full = kv_empty + KVS;   // 2
-  uint64_t* s_free = s_full + 2;                // 2 (128 arrivals)
-  uint64_t* p_ready = s_free + 2;               // 1 (128 arrivals)
-  uint64_t* p_free = p_ready + 1;               // 1
-  uint64_t* o_full = p_free + 1;                // 1
-  uint64_t* o_free = o_full + 1;                // 1 (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_free + 1);
+  uint64_t* kv_empty = kv_full + FA_KV_STAGES;
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = static_cast<int>(threadIdx.x) >> 5;
   const int q0 = blockIdx.x * 128;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int bkv = b / p.kv_batch_div;
-  const int nkv = (p.Lk + 127) / 128;
-  const bool bf16 = p.is_bf16 != 0;
+  const int nkv = (p.Lk + FA_BKV - 1) / FA_BKV;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmK);
     prefetch_tmap(&tmV);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      mbar_init(q_full, 1);
-      for (int i = 0; i < KVS; ++i) {
-        mbar_init(&kv_full[i], 1);
-        mbar_init(&kv_empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&s_free[i], 128);
-      }
-      mbar_init(p_ready, 128);
-      mbar_init(p_free, 1);
-      mbar_init(o_full, 1);
-      mbar_init(o_free, 128);
-      fence_barrier_init();
+    mbar_init(q_full, 1);
+    for (int i = 0; i < FA_KV_STAGES; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 8);         // lane 0 of each consumer warp
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, TCOLS);
-    tmem_relinquish();
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, FA_TILE_BYTES);
+      mbar_arrive_expect_tx(q_full, FA_Q_BYTES);
       tma_load_3d(smQ, &tmQ, q_full, p.q_col0 + head * 64, q0, b);
       for (int j = 0; j < nkv; ++j) {
-        const int s = j % KVS;
-        const uint32_t ph = (j / KVS) & 1;
-        mbar_wait(&kv_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&kv_full[s], 2 * FA_TILE_BYTES);
-        tma_load_3d(smK + s * FA_TILE_BYTES, &tmK, &kv_full[s], p.k_col0 + head * 64, j * 128, bkv);
-        tma_load_3d(smV + s * FA_TILE_BYTES, &tmV, &kv_full[s], p.v_col0 + head * 64, j * 128, bkv);
+        const int s = j % FA_KV_STAGES;
+        mbar_wait(&kv_empty[s], ((j / FA_KV_STAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * FA_KV_BYTES);
+        tma_load_3d(smK + s * FA_KV_BYTES, &tmK, &kv_full[s], p.k_col0 + head * 64, j * FA_BKV, bkv);
+        tma_load_3d(smV + s * FA_KV_BYTES, &tmV, &kv_full[s], p.v_col0 + head * 64, j * FA_BKV, bkv);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc_s = make_idesc_f16(bf16 ? 1 : 0, 128, 128, 0, 0);
-    const uint32_t idesc_o = make_idesc_f16(bf16 ? 1 : 0, 128, 64, 0, 1);   // B (=V) is MN-major
-    auto issue_s = [&](int jj) {
-      if (elect_one()) {
-        const uint32_t qa = smem_u32(smQ);
-        const uint32_t ka = smem_u32(smK + (jj % KVS) * FA_TILE_BYTES);
+    return;
+  }
+
+  const int cw = warp >> 2;                   // consumer warpgroup: query rows q0 + 64 cw ...
+  const int wq = warp & 3;
+  const int lane = static_cast<int>(lane_id());
+  const int row0 = 64 * cw + 16 * wq + (lane >> 2);     // tile rows row0 and row0 + 8
+  float o[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_f16_ss(tmem_base + (jj & 1) * 128, make_desc_kmajor_sw128(qa + k * 32),
-                      make_desc_kmajor_sw128(ka + k * 32), idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[jj & 1]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    mbar_wait(&kv_full[0], 0);
-    tc_fence_after();
-    issue_s(0);
-    for (int j = 0; j < nkv; ++j) {
-      if (j + 1 < nkv) {                      // S(j+1) into the other buffer while the softmax works on S(j)
-        mbar_wait(&kv_full[(j + 1) % KVS], ((j + 1) / KVS) & 1);
-        if (j >= 1) mbar_wait(&s_free[(j + 1) & 1], ((j - 1) >> 1) & 1);   // softmax(j-1) has read that buffer
-        tc_fence_after();
-        issue_s(j + 1);
-      }
-      mbar_wait(p_ready, j & 1);
-      if (j > 0) mbar_wait(o_free, (j - 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t pa = smem_u32(smP);
-        const uint32_t va = smem_u32(smV + (j % KVS) * FA_TILE_BYTES);
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t qa = smem_u32(smQ + cw * 64 * 128);
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < nkv; ++j) {
+    const int s = j % FA_KV_STAGES;
+    mbar_wait(&kv_full[s], (j / FA_KV_STAGES) & 1);
+    // ---------------- S = Q K^T   [64 x 64 keys]
+    float sc[32];
+    const uint32_t ka = smem_u32(smK + s * FA_KV_BYTES);
+    wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_f16_ss(tmem_base + O_COL, make_desc_kmajor_sw128(pa + (k >> 2) * FA_TILE_BYTES + (k & 3) * 32),
-                      make_desc_mnmajor_sw128(va + k * 2048, 8192), idesc_o, k > 0 ? 1u : 0u);
-        umma_commit(o_full);
-        umma_commit(p_free);
-        umma_commit(&kv_empty[j % KVS]);
+    for (int k = 0; k < 4; ++k)
+      wgmma_ss<64, BF16>(sc, make_desc_kmajor_sw128(qa + k * 32), make_desc_kmajor_sw128(ka + k * 32), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(sc);
+    // ---------------- mask keys past Lk (and, causal, past the query)
+    const int kbase = j * FA_BKV;
+    if (p.causal || p.Lk - kbase < FA_BKV) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int key = kbase + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        const int q = q0 + row0 + 8 * ((i >> 1) & 1);
+        if (key >= p.Lk || (p.causal && key > q)) sc[i] = -INFINITY;
       }
-      __syncwarp();
     }
-  } else {
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane_id();
-    const uint32_t lane_off = static_cast<uint32_t>(qd * 32) << 16;
-    const uint32_t t_o = tmem_base + O_COL + lane_off;
-    uint8_t* prow = smP + row * 128;
-    float o_acc[64];
+    // ---------------- online softmax on the two rows of this thread (a row's 64 keys live in the 4 lanes of a quad)
+    float alpha[2], m_new[2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) o_acc[i] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f, alpha_prev = 0.f;
-    auto accumulate = [&](int jj, float alpha) {        // o_acc = alpha * o_acc + O_jj
-      mbar_wait(o_full, jj & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_o + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o_acc[c * 32 + i] = fmaf(o_acc[c * 32 + i], alpha, __uint_as_float(r[i]));
-      }
-      tc_fence_before();
-      mbar_arrive(o_free);
-    };
-    for (int j = 0; j < nkv; ++j) {
-      const uint32_t t_s = tmem_base + (j & 1) * 128 + lane_off;
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      const int valid = p.Lk - j * 128;
-      const bool tail = valid < 128;
+    for (int h = 0; h < 2; ++h) {
       float mx = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + c * 32, r);
-        tmem_ld_wait();
-        if (!tail) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(r[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c * 32 + i < valid) mx = fmaxf(mx, __uint_as_float(r[i]));
-        }
-      }
-      const float m_new = fmaxf(m_run, mx * p.scale_log2);
-      const float alpha = fast_exp2(m_run - m_new);
-      m_run = m_new;
-      if (j > 0) mbar_wait(p_free, (j - 1) & 1);        // P.V of the previous block has consumed the P tile
-      float lsum = 0.f;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + c * 32, r);
-        tmem_ld_wait();
-        uint8_t* hp = prow + (c >> 1) * FA_TILE_BYTES;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float e[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float x = fast_exp2(fmaf(__uint_as_float(r[g * 8 + i]), p.scale_log2, -m_new));
-            if (tail && (c * 32 + g * 8 + i >= valid)) x = 0.f;
-            e[i] = x;
-            lsum += x;
-          }
-          uint4 u;
-          u.x = pack2(e[0], e[1], bf16);
-          u.y = pack2(e[2], e[3], bf16);
-          u.z = pack2(e[4], e[5], bf16);
-          u.w = pack2(e[6], e[7], bf16);
-          const int chunk = (c & 1) * 4 + g;
-          *reinterpret_cast<uint4*>(hp + ((chunk ^ (row & 7)) << 4)) = u;
-        }
-      }
-      l_run = l_run * alpha + lsum;
-      tc_fence_before();
-      mbar_arrive(&s_free[j & 1]);
-      fence_proxy_async_smem();
-      mbar_arrive(p_ready);
-      if (j > 0) accumulate(j - 1, alpha_prev);          // deferred read-back of the previous block's P.V
-      alpha_prev = alpha;
+      for (int i = 0; i < 32; ++i)
+        if (((i >> 1) & 1) == h) mx = fmaxf(mx, sc[i]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      m_new[h] = fmaxf(m_run[h], mx * p.scale_log2);
+      alpha[h] = fast_exp2(m_run[h] - m_new[h]);
+      m_run[h] = m_new[h];
     }
-    accumulate(nkv - 1, alpha_prev);
-    const int q = q0 + row;
-    if (q < p.Lq) {
-      const float inv = 1.0f / l_run;
-      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) +
-                                           (static_cast<long>(b) * p.out_batch_stride + static_cast<long>(q) * p.ld_out +
-                                            p.out_col0 + head * 64) * 2);
+    float lsum[2] = {0.f, 0.f};
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        uint4 u;
-        u.x = pack2(o_acc[g * 8 + 0] * inv, o_acc[g * 8 + 1] * inv, bf16);
-        u.y = pack2(o_acc[g * 8 + 2] * inv, o_acc[g * 8 + 3] * inv, bf16);
-        u.z = pack2(o_acc[g * 8 + 4] * inv, o_acc[g * 8 + 5] * inv, bf16);
-        u.w = pack2(o_acc[g * 8 + 6] * inv, o_acc[g * 8 + 7] * inv, bf16);
-        op[g] = u;
-      }
+    for (int i = 0; i < 32; ++i) {
+      const int h = (i >> 1) & 1;
+      sc[i] = fast_exp2(fmaf(sc[i], p.scale_log2, -m_new[h]));
+      lsum[h] += sc[i];
     }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + lsum[h];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    // ---------------- O += P V: P (16-bit) as the register A operand, 16 keys per wgmma
+    uint32_t pf[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      pf[kk][0] = pack2(sc[8 * kk + 0], sc[8 * kk + 1], BF16);
+      pf[kk][1] = pack2(sc[8 * kk + 2], sc[8 * kk + 3], BF16);
+      pf[kk][2] = pack2(sc[8 * kk + 4], sc[8 * kk + 5], BF16);
+      pf[kk][3] = pack2(sc[8 * kk + 6], sc[8 * kk + 7], BF16);
+    }
+    const uint32_t va = smem_u32(smV + s * FA_KV_BYTES);
+    fence_regs<32>(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs_tb<64, BF16>(o, pf[kk], make_desc_mnmajor_sw128(va + kk * 2048));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(o);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TCOLS);
+  // ---------------- normalise and store
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    const int q = q0 + row0 + 8 * h;
+    if (q < p.Lq) {
+      const float inv = 1.0f / l_run[h];
+      uint8_t* op = reinterpret_cast<uint8_t*>(p.out) +
+                    (static_cast<long>(b) * p.out_batch_stride + static_cast<long>(q) * p.ld_out + p.out_col0 + head * 64 +
+                     2 * (lane & 3)) * 2;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(op + jj * 16) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, BF16);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ temporal
 // q/k/v rows of frame t of (b, position pos): base + ((b*T + t)*HW + pos)*ld + col0 + head*64
-// One warp per (b, pixel, head).  T <= 32 is far below the 128-row tcgen05 tile, so the two tiny GEMMs
+// One warp per (b, pixel, head).  T <= 32 is far below the 64-row wgmma tile, so the two tiny GEMMs
 // (S = Q.K^T: 32x32x64, O = P.V: 32x64x32, T zero-padded to 32) run on warp-level mma.sync m16n8k16 with the online
 // softmax on the accumulator fragments (the S fragments are re-used as the A operand of P.V).  Q/K/V rows are gathered
 // with coalesced 8-byte loads into padded shared memory (row stride 144 B: conflict-free fragment loads).
@@ -826,8 +362,8 @@ temporal_attn_d64_kernel(const void* __restrict__ qkv, long ld, int q_col0, int 
 
 
 // ------------------------------------------------------------------------------------------------ temporal v2
-// Same math as temporal_attn_d64_kernel (bit-identical results), restructured for HBM throughput (round 2: the v1 kernel
-// reached 0.30 of the HBM roofline, profiles/r02_kernels_by_shape.md).  Persistent warps walk the (b, pixel, head) items;
+// Same math as temporal_attn_d64_kernel (bit-identical results), restructured for HBM throughput.  Persistent warps walk the
+// (b, pixel, head) items;
 // the Q/K/V rows of the NEXT item are fetched with 16-byte cp.async copies straight into the second shared-memory buffer
 // (408 copies in flight per warp, no registers involved) while the current item is computed; the normalised output is
 // staged in shared memory and written with 16-byte stores (one 128-byte row per 8 lanes).
@@ -1034,22 +570,21 @@ extern "C" int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, 
   if (!q || !kv || !out || lq < 1 || lk < 1 || heads < 1 || nb < 1 || kv_batch_div < 1) return AAB_ERR_ARG;
   if ((ldq % 8) || (ldkv % 8) || (ld_out % 8) || (out_col0 % 8)) return AAB_ERR_ARG;
   CUtensorMap tmQ, tmK, tmV;
-  int box[3] = {64, 128, 1};
   {
     long dims[3] = {q_cols, lq, nb};
     long strides[3] = {1, ldq, q_batch_stride};
+    int box[3] = {64, 128, 1};
     int r = make_tmap_16(&tmQ, q, 3, dims, strides, box, is_bf16);
     if (r) return r;
   }
   {
     long dims[3] = {kv_cols, lk, nb_kv};
     long strides[3] = {1, ldkv, kv_batch_stride};
+    int box[3] = {64, FA_BKV, 1};
     int r = make_tmap_16(&tmK, kv, 3, dims, strides, box, is_bf16);
     if (r) return r;
     tmV = tmK;
   }
-  static std::atomic<unsigned long long> attr_done{0};
-  if (int r = ensure_dyn_smem(flash_attn_d64_kernel, FA_SMEM_BYTES, attr_done)) return r;
   FaParams p;
   p.Lq = lq;
   p.Lk = lk;
@@ -1063,36 +598,16 @@ extern "C" int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, 
   p.out_batch_stride = out_batch_stride;
   p.out_col0 = out_col0;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.is_bf16 = is_bf16;
   p.causal = causal;
-  // Measured on B200 (nb=34, L=4096, 5 heads, bf16): v1 = 1.33 ms, v2 = 2.03 ms.  One softmax warpgroup per SM
-  // (v2) cannot hide its own tcgen05.ld / MUFU latencies; two warpgroups (v1) do, even though they wait for the MMAs in
-  // phase.  v1 is the default; AAB_FLASH_V2=1 selects v2 for experiments.
-  static int use_v1 = -1;
-  if (use_v1 < 0) {
-    const char* e = getenv("AAB_FLASH_V2");
-    use_v1 = (e && e[0] == '1') ? 0 : 1;
-  }
-  static int no_short = -1;               // AAB_FLASH_NO_SHORT=1: round-1 behaviour (A/B measurements)
-  if (no_short < 0) {
-    const char* e = getenv("AAB_FLASH_NO_SHORT");
-    no_short = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (lk <= 128 && !causal && !no_short) {      // one K/V block: the multi-CTA-per-SM variant
-    static std::atomic<unsigned long long> attr_s{0};
-    if (int r = ensure_dyn_smem(flash_attn_d64_v2_kernel<true>, FA2S_SMEM_BYTES, attr_s)) return r;
-    dim3 grid((lq + 127) / 128, heads, nb);
-    launch_k(flash_attn_d64_v2_kernel<true>, dim3(grid), dim3(FA2_THREADS), FA2S_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
-    return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
-  }
-  if (use_v1 || causal) {       // two query tiles per CTA (two softmax warpgroups), S single-buffered
-    dim3 grid((lq + 255) / 256, heads, nb);
-    launch_k(flash_attn_d64_kernel, dim3(grid), dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
+  const dim3 grid((lq + 127) / 128, heads, nb);
+  if (is_bf16) {
+    static std::atomic<unsigned long long> attr_b{0};
+    if (int r = ensure_dyn_smem(flash_attn_d64_kernel<true>, FA_SMEM_BYTES, attr_b)) return r;
+    launch_k(flash_attn_d64_kernel<true>, grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
   } else {
-    static std::atomic<unsigned long long> attr2_done{0};
-    if (int r = ensure_dyn_smem(flash_attn_d64_v2_kernel<false>, FA2_SMEM_BYTES, attr2_done)) return r;
-    dim3 grid((lq + 127) / 128, heads, nb);
-    launch_k(flash_attn_d64_v2_kernel<false>, dim3(grid), dim3(FA2_THREADS), FA2_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
+    static std::atomic<unsigned long long> attr_h{0};
+    if (int r = ensure_dyn_smem(flash_attn_d64_kernel<false>, FA_SMEM_BYTES, attr_h)) return r;
+    launch_k(flash_attn_d64_kernel<false>, grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }

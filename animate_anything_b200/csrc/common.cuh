@@ -1,6 +1,6 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 / TMEM.
-// All hand-written inline PTX; bit layouts of the UMMA descriptors follow the PTX ISA "tcgen05" chapter
-// (shared-memory matrix descriptor, instruction descriptor for .kind::f16).
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma).
+// All hand-written inline PTX; the bit layout of the wgmma shared-memory matrix descriptor follows the PTX ISA
+// "Asynchronous Warpgroup Level Matrix Multiply-Accumulate" chapter.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -77,15 +77,12 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return done != 0;
 }
-// Bounded wait: a protocol bug traps (sticky CUDA error) instead of hanging the GPU box.
+// Bounded wait: a protocol bug traps (sticky CUDA error) instead of hanging the GPU.  No printf here: a call inside a
+// kernel makes ptxas serialise the wgmma pipeline around it.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 24)) {
-      printf("aab: mbarrier timeout block %d thread %d bar %u parity %u\n", blockIdx.x, threadIdx.x,
-             smem_u32(bar), parity);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 
@@ -132,82 +129,59 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA store / UMMA operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2, cluster of 2)
-// Inside a 2-CTA cluster the shared::cluster address of the SAME smem offset in the even (leader) CTA is the own
-// shared::cta address with the peer bit (bit 24) cleared.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
+// ---------------------------------------------------------------- thread-block clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
+// every thread of every CTA of the cluster
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the LEADER CTA's copy of `bar` (callable from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-// TMA loads of a CTA pair: data lands in the executing CTA's smem, the transaction bytes are credited to the LEADER's barrier
-__device__ __forceinline__ void tma_load_5d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1),
-      "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs] * B[smem halves of both CTAs]: M = 256 (128 rows per CTA), issued by the leader
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
+// arrive on the copy of `bar` (same shared-memory offset) in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
       : "memory");
 }
-// arrive (once all previously issued MMAs of the pair completed) on the same-offset barrier of BOTH CTAs
-// arrive (once the MMAs issued so far have completed) on the copy of `bar` in every CTA of `cta_mask` (cluster ranks)
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask = 3) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
+// wait that also orders after arrivals released by the other CTAs of the cluster
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  for (;;) {
+    uint32_t done;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(done)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    if (done) return;
+    if (++spins > (1u << 26)) __trap();
+  }
 }
-// TMA load delivered to the same shared-memory offset of every CTA in `cta_mask`; each destination's transaction bytes are
-// credited to the LEADER of the destination's CTA pair (peer bit cleared in the barrier address)
-__device__ __forceinline__ void tma_load_3d_pair_mcast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                       uint16_t cta_mask) {
+// TMA load delivered to the same shared-memory offset of every CTA in `cta_mask`; each destination's bytes are credited to
+// the barrier at the same offset in that CTA
+__device__ __forceinline__ void tma_load_3d_mcast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
+                                                  uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%4, %5, %6}], [%2], %3;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "h"(cta_mask), "r"(c0),
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
       "r"(c1), "r"(c2)
       : "memory");
 }
@@ -217,102 +191,43 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], single CTA, kind::f16 (fp16 / bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i of the warp <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// same, 16 columns -> 16 registers
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes (64 x 16-bit) with the
-// 128-byte swizzle that TMA SWIZZLE_128B produces.  8-row groups are 1024 B apart (SBO); LBO is unused for
-// swizzled K-major layouts.  Bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1,
-// [61,64) layout (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;            // LBO (ignored)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
-  return d;
-}
-// MN-major operand (the MN index is contiguous): tile stored as rows of 128 bytes where a row is one K index and
-// holds 64 consecutive MN elements; 8-row (8 x K) groups are 1024 B apart (SBO); LBO = byte distance between
-// 64-element MN chunks (only used when the MN extent of the MMA exceeds 64).
-__device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor of an operand tile stored as rows of 128 bytes (64 x 16-bit) with the 128-byte swizzle
+// that TMA SWIZZLE_128B produces; 8-row groups are 1024 B apart.  Bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4,
+// [62,64) layout (1 = SWIZZLE_128B).  K-major (K contiguous in a row): SBO = 1024, LBO unused; a K step of 16 elements
+// advances the start address by 32 bytes inside the swizzle atom.  MN-major (a row is one K index holding 64 consecutive
+// MN elements): 8-row K groups are 1024 B apart and an MN extent of 64 needs no second chunk, so both offsets are 1024.
+__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
+__device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) { return make_desc_sw128(smem_addr, 16); }
+__device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr) { return make_desc_sw128(smem_addr, 1024); }
 
-// Instruction descriptor, .kind::f16: D fp32; A/B fp16 (0) or bf16 (1); K-major unless *_mn set.
-__host__ __device__ inline uint32_t make_idesc_f16(int is_bf16, int M, int N, int a_mn, int b_mn) {
-  uint32_t d = 0;
-  d |= 1u << 4;                                   // c_format = F32
-  d |= static_cast<uint32_t>(is_bf16 ? 1 : 0) << 7;   // a_format
-  d |= static_cast<uint32_t>(is_bf16 ? 1 : 0) << 10;  // b_format
-  d |= static_cast<uint32_t>(a_mn ? 1 : 0) << 15;
-  d |= static_cast<uint32_t>(b_mn ? 1 : 0) << 16;
-  d |= static_cast<uint32_t>(N >> 3) << 17;
-  d |= static_cast<uint32_t>(M >> 4) << 24;
-  return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points
+template <int N>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// register budget of a warpgroup (producer warpgroups give registers to the accumulator-holding consumers)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
 }
 
 // ---------------------------------------------------------------- host: per-device opt-in to > 48 KiB dynamic smem
@@ -335,10 +250,8 @@ inline int ensure_dyn_smem(Kernel kernel, int bytes, std::atomic<unsigned long l
 //                                       has started (its CTAs take the SM resources this grid frees while draining);
 //   pdl_wait()     before the first global-memory access (read OR write) -- blocks until the PREVIOUS grid has completed
 //                                       and its memory is visible.
-// So only set-up work (barrier init, TMEM allocation, descriptor prefetch, index math) overlaps the predecessor's tail;
-// data hazards are impossible by construction.  Measured in round 2 (profiles/r02_pdl_ab.md, same box, all 135 GPU tests green
-// with it on): 5.214 frames/s with, 5.229 without -- the persistent kernels leave no gap worth hiding, so it is OFF by
-// default (launches carry no attribute and both calls are no-ops); AAB_PDL=1 enables it.
+// So only set-up work (barrier init, descriptor prefetch, index math) overlaps the predecessor's tail; data hazards are
+// impossible by construction.  Off by default (launches carry no attribute and both calls are no-ops); AAB_PDL=1 enables it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM on tcgen05 tensor cores for every dense contraction of the denoising path:
+// Implicit-GEMM on the Hopper warpgroup MMA (wgmma) for every dense contraction of the denoising path:
 //   Linear / 1x1 conv (1 tap), conv3x3 (9 taps over H,W), temporal conv (3,1,1) (3 taps over T),
 //   stride-2 conv (9 taps over a space-to-depth view), batched Q.K^T / P.V for the VAE attention.
 //
@@ -7,60 +7,45 @@
 // * A (activations, channels-last) is never im2col'd: every tap is a TMA box load of the same 5-D tensor map at a
 //   shifted pixel coordinate; out-of-bounds pixels are zero-filled by the TMA unit (= conv zero padding).
 // * B (weights, [N, K] K-contiguous) is TMA-loaded; both land in shared memory in the 128B-swizzled K-major layout
-//   that tcgen05.mma consumes directly.  One elected thread issues tcgen05.mma (M=128, N=BN, K=16), accumulators
-//   live in TMEM (double buffered so the epilogue of tile i overlaps the main loop of tile i+1).
+//   that wgmma reads through matrix descriptors.  A stage ring of mbarrier-guarded buffers feeds the tensor cores.
+// * Warp specialisation: warpgroup 0 is the TMA producer (one elected thread), warpgroups 1 and 2 each own 64 rows of
+//   the 128 x BN tile and keep their accumulators in registers (m64nBNk16 wgmma, fp32).
 // * Persistent CTAs (one per SM) walk the tile list n-fastest so that the CTAs running concurrently share the same
-//   A rows (L2 hits) while the weights stay L2-resident.
-// * Epilogue warps: tcgen05.ld -> bias / per-sample bias (time embedding) / residual / activation / GEGLU gate ->
-//   16-bit pack -> swizzled smem staging -> TMA store (hardware clips partial tiles).  A direct-store variant handles
-//   N that is not a multiple of 8 (e.g. conv_out, N=4) and fp32 outputs.
+//   A rows (L2 hits) while the weights stay L2-resident; the producer runs ahead into the next tile while the
+//   consumers finish the epilogue of the current one.
+// * Clusters (IgemmParams::cluster = 2 or 4, 256-column tiles): the CTAs of a cluster take consecutive m-tiles of the same
+//   n-tile; each fetches 1/cluster of the weight tile and multicasts it to all of them, so a k-block reads the weights from
+//   L2 once per cluster instead of once per CTA.  A stage is refilled only after the consumers of every CTA of the cluster
+//   have released it.  Same K order, same epilogue: bit-identical to single CTAs.
+// * Epilogue straight from the accumulator registers: bias / per-sample bias (time embedding) / residual / activation
+//   / GEGLU gate -> 16-bit (or fp32) stores, masked at the tile edges, plus optional per-tile column statistics for the
+//   GroupNorm that follows.
 //
 // Replaces, for the reference path (SURVEY.md section 8a): cuDNN conv2d/conv3d and cuBLAS linear calls made by
 // diffusers ResnetBlock2D / TemporalConvLayer / Transformer2DModel / TransformerTemporalModel / AutoencoderKL
 // (models/unet_3d_blocks.py:262-306,425-467,564-583,660-701,794-813).
 #include "common.cuh"
 #include "igemm.h"
+#include "wgmma.cuh"
 
 namespace aab {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;       // 16 KiB
-constexpr int OUT_CHUNK_BYTES = BM * 32 * 2;     // one 32-column output chunk (64-byte rows, SWIZZLE_64B), 8 KiB
-constexpr int NUM_EPI_GROUPS = 4;                // epilogue warpgroups (4 warps each): latency-bound chains, so more in parallel
-constexpr int NUM_THREADS = 32 * (2 + 4 * NUM_EPI_GROUPS);  // warp0 TMA, warp1 MMA, warps 2..17 epilogue
+constexpr int NUM_CONSUMERS = 2;                 // consumer warpgroups, 64 tile rows each
+constexpr int NUM_THREADS = 128 * (1 + NUM_CONSUMERS);
+constexpr int NUM_CONSUMER_WARPS = 4 * NUM_CONSUMERS;
 
-// smem ring depth per tile width: 192 KiB of operands in flight whatever BN
-// PAIR (cta_group::2): a cluster of two CTAs computes a 256 x BN tile with ONE tcgen05.mma per K=16 step; each CTA stages its
-// own 128 activation rows and HALF of the weight tile (BN/2 rows), so a stage is 32 KiB instead of 48 and the MMA reads a third
-// less shared memory per FLOP (measured, profiles/r02_umma_rate.log: single-CTA SS-mode N=256 runs at 171 clk per K=16
-// instruction = 75 % of the tensor peak whatever the pipeline does).
-template <int BN, bool PAIR = false>
+// smem ring depth per tile width: 192 KiB (160 KiB for BN = 32) of operands in flight whatever BN, plus the column-statistics
+// scratch, inside the 227 KiB a block may use
+template <int BN>
 struct Cfg {
-  static constexpr int STAGES = PAIR ? 6 : (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
-  static constexpr int B_STAGE_BYTES = (PAIR ? BN / 2 : BN) * BK * 2;
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;   // two accumulator stages
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 4 /*epilogue groups*/ * OUT_CHUNK_BYTES +
-                                    1024 /*align*/ + 512 /*barriers*/;
-};
-
-// profiling aid: cycles spent inside an mbarrier wait, accumulated per warp role when IgemmParams::dbg != NULL
-struct WaitTimer {
-  unsigned long long acc = 0;
-  bool on;
-  __device__ explicit WaitTimer(const void* dbg) : on(dbg != nullptr) {}
-  __device__ __forceinline__ void wait(uint64_t* bar, uint32_t parity) {
-    if (on) {
-      const long long t0 = clock64();
-      mbar_wait(bar, parity);
-      acc += static_cast<unsigned long long>(clock64() - t0);
-    } else {
-      mbar_wait(bar, parity);
-    }
-  }
-  __device__ __forceinline__ void flush(unsigned long long* dbg, int slot) {
-    if (on) atomicAdd(dbg + slot, acc);
-  }
+  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
+  static constexpr int STATS_BYTES = NUM_CONSUMER_WARPS * BN * 2 * 4;   // per-warp (sum, sum of squares) per column
+  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + STATS_BYTES + 1024 /*align*/ +
+                                    256 /*barriers*/;
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -70,106 +55,81 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-// EPI (compile-time epilogue variant; the hot loop of each variant is straight-line code):
-//      0 = + bias                                  -> 16-bit, swizzled smem staging + TMA store (n_out % 32 == 0)
-//      1 = GEGLU gate (B tile = [values | gates], out = value * gelu(gate))
-//      2 = generic direct-to-global store (any n_out, fp32 / 16-bit output, masked, any flag combination)
-//      3 = + bias + residual       4 = + bias + per-sample bias (time embedding)       5 = + bias, SiLU
-// The epilogue is written as compact loops (no full unrolling): its instruction footprint is executed once per tile by
-// four warps, and a bloated epilogue thrashes the instruction cache when K is small.
-template <int BN, int EPI, bool PAIR = false>
+template <int BN, bool BF16>
+__device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_addr, uint32_t b_addr, bool first) {
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t da = make_desc_kmajor_sw128(a_addr + k * 32);
+    const uint64_t db = make_desc_kmajor_sw128(b_addr + k * 32);
+    const uint32_t sc = (first && k == 0) ? 0u : 1u;
+    wgmma_ss<BN, BF16>(acc, da, db, sc);
+  }
+}
+
+// GEGLU: B tile = [values | gates] (BN/2 rows each), out = value * gelu(gate), BN/2 columns.
+// Epilogue flavours (runtime, uniform per launch):
+//   staged  (no AAB_F_DIRECT): n_out % 32 == 0, 16-bit output, at most one of residual / per-sample bias / SiLU, no scaling;
+//                              column pairs are stored as 32-bit words; may emit column statistics
+//   direct  (AAB_F_DIRECT):    any n_out, fp32 or 16-bit output, every flag combination, masked per element
+template <int BN, bool GEGLU, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-             const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
-             const __grid_constant__ CUtensorMap tmR, const IgemmParams p) {
+             const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
   pdl_trigger();
-  using C = Cfg<BN, PAIR>;
-  static_assert(!PAIR || BN == 256, "the CTA-pair variant is built for 256-column tiles");
-  constexpr int STAGES = C::STAGES;
-  constexpr bool GEGLU = (EPI == 1);
+  using CF = Cfg<BN>;
+  constexpr int STAGES = CF::STAGES;
   constexpr int OUT_BN = GEGLU ? BN / 2 : BN;
-  constexpr bool HAS_RES = (EPI == 3);
-  constexpr bool HAS_BIAS2 = (EPI == 4);
-  constexpr bool HAS_SILU = (EPI == 5);
-  constexpr bool DIRECT = (EPI == 2);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smA = smem;
   uint8_t* smB = smA + STAGES * A_STAGE_BYTES;
-  uint8_t* smO = smB + STAGES * C::B_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smO + NUM_EPI_GROUPS * OUT_CHUNK_BYTES);
+  float* sstats = reinterpret_cast<float*>(smB + STAGES * CF::B_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sstats) + CF::STATS_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
-  const int warp = threadIdx.x >> 5;
-  const bool bf16 = (p.flags & AAB_F_BF16) != 0;
-  // PAIR: the two CTAs of a cluster walk the same list of PAIR tiles (two consecutive m-tiles x one n-tile); CTA rank r owns
-  // m-tile 2 * pm + r.  With an odd number of m-tiles the last pair's second m-tile does not exist: rank 1 then recomputes
-  // m-tile 0 (coordinates wrap) and its epilogue stores nothing.
-  // QUAD (p.cluster == 4, runtime): two pairs stacked along M share every weight tile -- each CTA fetches HALF of its pair-half
-  // (64 rows) and multicasts it to the CTA of the same pair rank in the other pair, so a k-block costs 24 KB of L2 reads per
-  // CTA instead of 32 KB (the L2 -> shared-memory feed is what paces this kernel, profiles/r02_igemm_split_issue.md).
-  const uint32_t clrank = PAIR ? cluster_ctarank() : 0u;        // rank in the cluster: m-tile offset inside the cluster tile
-  const uint32_t crank = clrank & 1u;                            // rank in the CTA pair (0 = leader, issues the MMAs)
-  const uint32_t qrank = clrank >> 1;                            // which pair of the cluster
-  const int CL = PAIR ? p.cluster : 1;
-  const bool quad = PAIR && CL == 4;
+  const int wg = static_cast<int>(threadIdx.x) >> 7;
+  const int warp = static_cast<int>(threadIdx.x) >> 5;
+  constexpr bool bf16 = BF16;
+  // cluster tiles: CL consecutive m-tiles x one n-tile; this CTA owns m-tile CL * (tile / num_n_tiles) + crank.  With a
+  // number of m-tiles that CL does not divide, the CTAs past the end load m-tile 0 (the cluster moves in lockstep) and
+  // store nothing.
+  const int CL = p.cluster;
+  const int crank = CL > 1 ? static_cast<int>(cluster_ctarank()) : 0;
   const int tile_first = static_cast<int>(blockIdx.x) / CL;
   const int tile_step = static_cast<int>(gridDim.x) / CL;
   const int num_tiles = ((p.num_m_tiles + CL - 1) / CL) * p.num_n_tiles;
   const int kb_per_tap = p.kb_per_tap;
   const int k_iters = p.num_taps * kb_per_tap;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmA2);
     prefetch_tmap(&tmB);
-    prefetch_tmap(&tmD);
-    prefetch_tmap(&tmR);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int i = 0; i < STAGES; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], quad ? 2 : 1);   // QUAD: a stage is refilled by two CTAs' loads, read by two pairs' MMAs
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull_bar[i], 1);
-        // PAIR: the leader's MMA thread waits for the epilogue WARPS of both CTAs (one remote arrival per warp: 32 per
-        // accumulator stage instead of 1024 per-thread arrivals crossing the pair link)
-        mbar_init(&tempty_bar[i], PAIR ? 2 * 4 * NUM_EPI_GROUPS : 128 * NUM_EPI_GROUPS);
-      }
-      fence_barrier_init();
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], NUM_CONSUMER_WARPS * CL);   // lane 0 of every consumer warp of the cluster releases a stage
     }
-    __syncwarp();
-    if (PAIR) {
-      tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish();
-    }
+    fence_barrier_init();
   }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();     // the peer's barriers must be initialised before anything is signalled across the pair
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();       // everything above (barriers, TMEM, descriptor prefetch) overlapped the previous kernel's tail
+  __syncthreads();
+  if (CL > 1) cluster_sync_all();     // the other CTAs' barriers are initialised before anything is signalled into them
+  pdl_wait();       // everything above (barriers, descriptor prefetch) overlapped the previous kernel's tail
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================================== TMA producer
-    if (elect_one()) {
-      WaitTimer w_empty(p.dbg);
-      const long long t_start = clock64();
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // the weight tile is fetched in NS row slices of BN / NS rows (GEGLU: values and gates are separate slices); CTA crank
+      // of the cluster fetches slices crank, crank + CL, ... and multicasts them
+      const int NS = (CL > 1 || !GEGLU) ? CL : 2;
+      const int slice_rows = BN / (NS > 1 ? NS : 1);
+      const uint16_t mask = static_cast<uint16_t>((1u << CL) - 1u);
       uint32_t it = 0;
       for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
         const int nt = tile % p.num_n_tiles;
-        int mt = tile / p.num_n_tiles;
-        if (PAIR) mt = CL * mt + static_cast<int>(clrank);
+        int mt = (tile / p.num_n_tiles) * CL + crank;
+        if (mt >= p.num_m_tiles) mt = 0;
         int cb[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -178,473 +138,230 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         }
         const int bbatch = (p.b_batch_dim >= 0) ? cb[p.b_batch_dim] : 0;
         const int n0 = nt * OUT_BN;
-        // PAIR: this CTA stages rows [crank * n_mma / 2, (crank + 1) * n_mma / 2) of the weight tile (n_mma = valid columns
-        // rounded up to 32); for GEGLU rank 0 holds the value rows and rank 1 the gate rows
-        int nb0 = n0, bq_off = 0;
-        if (PAIR && !GEGLU) {
-          int nv = p.N - n0;
-          nv = nv < BN ? ((nv + 31) & ~31) : BN;
-          nb0 = n0 + static_cast<int>(crank) * (nv / 2);
-          if (quad) nb0 += static_cast<int>(qrank) * (nv / 4);     // this CTA's quarter; lands nv/4 rows into the stage
-          bq_off = static_cast<int>(qrank) * (nv / 4) * 128;
-        }
-        if (PAIR && GEGLU) {
-          nb0 = (crank ? p.N / 2 : 0) + n0 + (quad ? static_cast<int>(qrank) * 64 : 0);
-          bq_off = quad ? static_cast<int>(qrank) * 64 * 128 : 0;
-        }
-        const uint16_t bq_mask = static_cast<uint16_t>((1u << crank) | (1u << (crank + 2)));   // same pair rank, both pairs
         for (int tap = 0; tap < p.num_taps; ++tap) {
           const int o0 = p.tap_off[tap][0], o1 = p.tap_off[tap][1], o2 = p.tap_off[tap][2], o3 = p.tap_off[tap][3],
                     o4 = p.tap_off[tap][4];
           for (int kb = 0; kb < kb_per_tap; ++kb, ++it) {
             const int s = it % STAGES;
             const uint32_t ph = (it / STAGES) & 1;
-            if (!(p.flags & AAB_F_DBG_NO_SYNC)) w_empty.wait(&empty_bar[s], ph ^ 1);
-#ifdef AAB_IGEMM_TRACE
-            if (p.dbg && blockIdx.x == 0 && it < 96) p.dbg[16 + it] = static_cast<unsigned long long>(clock64());
-#endif
-            if (p.flags & AAB_F_DBG_NO_LOAD) {
-              if (!(p.flags & AAB_F_DBG_NO_SYNC)) mbar_arrive(&full_bar[s]);
-              continue;
-            }
+            mbar_wait_cluster(&empty_bar[s], ph ^ 1);
             const int kc = kb * BK;
             const int kg = tap * p.Kc + kc;
-            if (PAIR) {
-              // one expect_tx for the bytes of BOTH CTAs on the leader's barrier; every load of the pair is credited there
-              if (crank == 0) mbar_arrive_expect_tx(&full_bar[s], 2 * (A_STAGE_BYTES + C::B_STAGE_BYTES));
-              if (kc < p.Kc1)
-                tma_load_5d_pair(smA + s * A_STAGE_BYTES, &tmA, &full_bar[s], kc + o0, cb[0] + o1, cb[1] + o2, cb[2] + o3,
-                                 cb[3] + o4);
-              else
-                tma_load_5d_pair(smA + s * A_STAGE_BYTES, &tmA2, &full_bar[s], kc - p.Kc1 + o0, cb[0] + o1, cb[1] + o2,
-                                 cb[2] + o3, cb[3] + o4);
-              if (quad)     // 64-row box (8 KB) to this CTA and to its twin in the other pair; the twin sends the other one
-                tma_load_3d_pair_mcast(smB + s * C::B_STAGE_BYTES + bq_off, &tmB, &full_bar[s], kg, nb0, bbatch, bq_mask);
-              else
-                tma_load_3d_pair(smB + s * C::B_STAGE_BYTES, &tmB, &full_bar[s], kg, nb0, bbatch);
-              continue;
-            }
-            mbar_arrive_expect_tx(&full_bar[s], A_STAGE_BYTES + C::B_STAGE_BYTES);
+            mbar_arrive_expect_tx(&full_bar[s], A_STAGE_BYTES + CF::B_STAGE_BYTES);
             if (kc < p.Kc1)
               tma_load_5d(smA + s * A_STAGE_BYTES, &tmA, &full_bar[s], kc + o0, cb[0] + o1, cb[1] + o2, cb[2] + o3,
                           cb[3] + o4);
             else
               tma_load_5d(smA + s * A_STAGE_BYTES, &tmA2, &full_bar[s], kc - p.Kc1 + o0, cb[0] + o1, cb[1] + o2,
                           cb[2] + o3, cb[3] + o4);
-            tma_load_3d(smB + s * C::B_STAGE_BYTES, &tmB, &full_bar[s], kg, n0, bbatch);
-            if (GEGLU)
-              tma_load_3d(smB + s * C::B_STAGE_BYTES + (BN / 2) * 128, &tmB, &full_bar[s], kg, p.N / 2 + n0, bbatch);
+            for (int j = crank; j < (NS > 1 ? NS : 1); j += CL) {
+              const int t0 = j * slice_rows;                        // first tile row of the slice
+              const int row = (GEGLU && t0 >= BN / 2) ? p.N / 2 + n0 + (t0 - BN / 2) : n0 + t0;
+              uint8_t* dst = smB + s * CF::B_STAGE_BYTES + t0 * 128;
+              if (CL > 1) tma_load_3d_mcast(dst, &tmB, &full_bar[s], kg, row, bbatch, mask);
+              else tma_load_3d(dst, &tmB, &full_bar[s], kg, row, bbatch);
+            }
           }
         }
       }
-      w_empty.flush(p.dbg, 0);                                  // slot 0: producer waiting for a free stage
-      if (p.dbg) atomicAdd(p.dbg + 15, static_cast<unsigned long long>(clock64() - t_start));   // slot 15: producer lifetime
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer: ONE elected thread runs the whole loop.
-    // Measured (profiles/r01_igemm_issue_trace.md): with "wait full -> 4 x tcgen05.mma -> commit" per k-block the
-    // issuing thread needed ~750 clk per k-block where the tensor pipe needs ~590 (raw issue rate): the blocking
-    // mbarrier wait sat between two k-blocks' MMAs and let the pipe's short queue run dry.  So the NEXT stage's full
-    // barrier is peeked (non-blocking test_wait) in the middle of the current k-block's MMAs; when it is already
-    // complete -- the common case -- the next k-block's MMAs follow back to back.
-    if ((!PAIR || crank == 0) && elect_one()) {      // PAIR: only the leader CTA issues (for both)
-      WaitTimer w_full(p.dbg), w_tempty(p.dbg);
-      const bool nosync = (p.flags & AAB_F_DBG_NO_SYNC) != 0;
-      const bool nomma = (p.flags & AAB_F_DBG_NO_MMA) != 0;
-#ifdef AAB_IGEMM_TRACE
-      const bool trace = p.dbg != nullptr && blockIdx.x == 0;
-#endif
-      uint32_t it = 0;
-      uint32_t tl = 0;
-      bool ready = false;   // full barrier of k-block `it` already observed complete
-      for (int tile = tile_first; tile < num_tiles; tile += tile_step, ++tl) {
-        const uint32_t as = tl & 1;
-        const uint32_t aph = (tl >> 1) & 1;
-        // ragged last N tile: issue the MMA only over the valid columns (multiple of 16; 32 for a CTA pair, which splits
-        // them between its two CTAs); the TMA box of B is zero-filled beyond N, so no extra traffic either.
-        int n_mma = BN;
-        if (!GEGLU) {
-          const int nvalid = p.N - (tile % p.num_n_tiles) * BN;
-          if (nvalid < BN) n_mma = PAIR ? ((nvalid + 31) & ~31) : ((nvalid + 15) & ~15);
-        }
-        // (Splitting the tile into two column halves issued alternately -- so that consecutive tcgen05.mma never accumulate into
-        // the same TMEM columns, which a bare issue loop rewards with N/2 instead of N/2 + 43 clk per instruction,
-        // profiles/r02_umma_rate_v3.log -- was built and measured for single CTAs and for pairs: 2-5 % SLOWER on every large
-        // shape (profiles/r02_igemm_split_issue.md).  The tensor pipe is not what paces this kernel; the operand feed is.)
-        const uint32_t idesc = make_idesc_f16(bf16 ? 1 : 0, PAIR ? 2 * BM : BM, n_mma, 0, 0);
-        w_tempty.wait(&tempty_bar[as], aph ^ 1);
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int ki = 0; ki < k_iters; ++ki, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          if (!nosync && !ready) w_full.wait(&full_bar[s], ph);
-          tc_fence_after();
-#ifdef AAB_IGEMM_TRACE
-          if (trace && it < 96) p.dbg[16 + 96 + it] = static_cast<unsigned long long>(clock64());
-#endif
-          const int s1 = (it + 1) % STAGES;
-          const uint32_t ph1 = ((it + 1) / STAGES) & 1;
-          if (nomma) {
-            mbar_arrive(&empty_bar[s]);
-            if (ki == k_iters - 1) mbar_arrive(&tfull_bar[as]);
-            ready = false;
-            continue;
-          }
-          const uint32_t a_addr = smem_u32(smA + s * A_STAGE_BYTES);
-          const uint32_t b_addr = smem_u32(smB + s * C::B_STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = make_desc_kmajor_sw128(a_addr + k * 32);
-            const uint64_t db = make_desc_kmajor_sw128(b_addr + k * 32);
-            if (PAIR) umma_f16_ss_pair(tmem_d, da, db, idesc, (ki > 0 || k > 0) ? 1u : 0u);
-            else umma_f16_ss(tmem_d, da, db, idesc, (ki > 0 || k > 0) ? 1u : 0u);
-            if (k == BK / 32 - 1) ready = !nosync && !(p.flags & AAB_F_DBG_NO_PEEK) && mbar_test_wait(&full_bar[s1], ph1);
-          }
-          if (PAIR) {                       // release the stage (QUAD: in all four CTAs) / publish the accumulator in BOTH CTAs
-            umma_commit_pair(&empty_bar[s], quad ? static_cast<uint16_t>(15) : static_cast<uint16_t>(3));
-            if (ki == k_iters - 1) umma_commit_pair(&tfull_bar[as], static_cast<uint16_t>(3u << (2 * qrank)));
-          } else {
-            if (!nosync) umma_commit(&empty_bar[s]);
-            if (ki == k_iters - 1) umma_commit(&tfull_bar[as]);
-          }
-#ifdef AAB_IGEMM_TRACE
-          if (trace && it < 96) p.dbg[16 + 192 + it] = static_cast<unsigned long long>(clock64());
-#endif
-        }
-      }
-      w_full.flush(p.dbg, 1);                                   // slot 1: MMA waiting for TMA data
-      w_tempty.flush(p.dbg, 2);                                 // slot 2: MMA waiting for a drained accumulator
+    if (CL > 1) {                     // no CTA leaves while a peer may still multicast into it or release its stages
+      __syncwarp();
+      cluster_sync_all();
     }
-    __syncwarp();
-  } else {
-    // ===================================================== epilogue: warps 2..17 = four independent groups of four warps
-    // (TMEM lane quarter = warp % 4).  Group eg owns the 32-column chunks with (chunk index % 4 == eg) of every tile, ONE
-    // private 8 KiB staging buffer (64-byte rows, SWIZZLE_64B) and its own TMA-store bulk groups, so no group ever waits
-    // for another one: the drain of its previous store (~350 clk, measured) overlaps the TMEM load + math of its next
-    // chunk.  The accumulator stage is handed back to the MMA warp right after the group's last TMEM read of the tile.
-    const int q = warp & 3;
-    const int eg = (warp - 2) >> 2;
-    const int row = q * 32 + lane_id();           // row inside the 128-row tile == TMEM lane
-    const bool leader = (q == 2) && (lane_id() == 0);   // first thread of the group's first warp (warp 2 + 4 eg)
-    constexpr int CPT = OUT_BN / 32;              // chunks per tile
-    uint8_t* stage_buf = smO + eg * OUT_CHUNK_BYTES;
-    uint8_t* rowp = stage_buf + row * 64;         // this thread's 64-byte row; 16-byte piece c at ((c ^ sw) << 4)
-    const int sw = (row >> 1) & 3;
-    const uint32_t bar_id = 1 + eg;
-    uint32_t tl = 0;
-    WaitTimer w_tfull(p.dbg);
-    unsigned long long t_bar = 0, t_math = 0;
+    return;
+  }
 
-    auto prefetch_res_tile = [&](long tile2) {    // residual rows -> L2, one tile ahead (leader of group 0 only)
-      if (tile2 >= num_tiles) return;
-      const int nt2 = static_cast<int>(tile2 % p.num_n_tiles);
-      int mt2 = static_cast<int>(tile2 / p.num_n_tiles);
-      int c2[4];
+  // ===================================================== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64)
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;
+  const int wq = warp & 3;
+  const int lane = static_cast<int>(lane_id());
+  const bool direct = (p.flags & AAB_F_DIRECT) != 0;
+  const bool out_f32 = (p.flags & AAB_F_OUT_F32) != 0;
+  const bool scale_acc = (p.flags & AAB_F_SCALE_ACC) != 0;
+  const bool stats = !GEGLU && !direct && p.colstats != nullptr;
+  uint32_t it = 0;
+
+  auto release = [&](uint32_t stage) {
+    if (lane != 0) return;
+    if (CL > 1) {
+      for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&empty_bar[stage], static_cast<uint32_t>(r));
+    } else {
+      mbar_arrive(&empty_bar[stage]);
+    }
+  };
+
+  for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
+    float acc[BN / 2];                  // the first wgmma of a tile overwrites it (scale-d = 0)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // ---------------- main loop: one k-block of wgmmas in flight while the previous one retires and frees its stage
+    for (int ki = 0; ki < k_iters; ++ki, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full_bar[s], (it / STAGES) & 1);
+      fence_regs<BN / 2>(acc);
+      wgmma_fence();
+      mma_kblock<BN, BF16>(acc, smem_u32(smA + s * A_STAGE_BYTES + cw * 64 * 128),
+                           smem_u32(smB + s * CF::B_STAGE_BYTES), ki == 0);
+      wgmma_commit();
+      fence_regs<BN / 2>(acc);
+      if (ki > 0) {
+        wgmma_wait<1>();
+        fence_regs<BN / 2>(acc);
+        release((it - 1) % STAGES);
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs<BN / 2>(acc);
+    release((it - 1) % STAGES);
+
+    // ---------------- epilogue
+    const int nt = tile % p.num_n_tiles;
+    int mt = (tile / p.num_n_tiles) * CL + crank;
+    const bool tile_ok = mt < p.num_m_tiles;                 // a cluster CTA past the last m-tile stores nothing
+    if (!tile_ok) mt = 0;
+    const int mt_lin = mt;                                  // linear m-tile index (row of the column-statistics table)
+    int cb[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      cb[i] = (mt % p.tiles[i]) * p.box[i];
+      mt /= p.tiles[i];
+    }
+    // this thread's two accumulator rows: r and r + 8 of the tile
+    long grow[2];
+    bool rvalid[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      int rr = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      int g[4];
+      bool v = true;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        c2[i] = (mt2 % p.tiles[i]) * p.box[i];
-        mt2 /= p.tiles[i];
+        g[i] = cb[i] + rr % p.box[i];
+        rr /= p.box[i];
+        v = v && (g[i] < p.dimD[i]);
       }
-      for (int ci = 0; ci < CPT; ++ci) {
-        const int col2 = nt2 * OUT_BN + ci * 32;
-        if (col2 < p.n_out) tma_prefetch_l2_5d(&tmR, col2, c2[0], c2[1], c2[2], c2[3]);
-      }
-    };
-    const bool do_prefetch = !PAIR && HAS_RES && p.residual != nullptr && leader && eg == 0;
-    if (do_prefetch) prefetch_res_tile(blockIdx.x);
+      rvalid[h] = v && tile_ok;
+      grow[h] = ((static_cast<long>(g[3]) * p.dimD[2] + g[2]) * p.dimD[1] + g[1]) * p.dimD[0] + g[0];
+    }
+    const int n0 = nt * OUT_BN;
+    const float* bias2row[2];
+    const uint8_t* resrow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      bias2row[h] = (p.bias2 != nullptr && rvalid[h]) ? p.bias2 + (grow[h] / p.rows_per_bias2) * p.ld_bias2 : nullptr;
+      resrow[h] = (p.residual != nullptr && rvalid[h])
+                      ? reinterpret_cast<const uint8_t*>(p.residual) + grow[h] * p.ld_res * 2
+                      : nullptr;
+    }
+    if (stats) named_bar_sync(1, 128 * NUM_CONSUMERS);     // the previous tile's statistics scratch has been read
 
-    for (int tile = tile_first; tile < num_tiles; tile += tile_step, ++tl) {
-      const uint32_t as = tl & 1;
-      const uint32_t aph = (tl >> 1) & 1;
-      const int nt = tile % p.num_n_tiles;
-      int mt = tile / p.num_n_tiles;
-      if (PAIR) mt = CL * mt + static_cast<int>(clrank);
-      const bool tile_ok = !PAIR || mt < p.num_m_tiles;      // PAIR, odd m-tile count: rank 1 of the last pair stores nothing
-      const int mt_lin = mt;                                  // linear m-tile index (row of the column-statistics table)
-      int cb[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        cb[i] = (mt % p.tiles[i]) * p.box[i];
-        mt /= p.tiles[i];
-      }
-      long grow = 0;
-      bool rvalid = true;
-      {
-        int rr = row;
-        int g[4];
+    for (int jj = 0; jj < OUT_BN / 8; ++jj) {
+      const int cl = jj * 8 + 2 * (lane & 3);                // tile column of this thread's pair
+      const int col = n0 + cl;
+      float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          g[i] = cb[i] + rr % p.box[i];
-          rr /= p.box[i];
-          rvalid = rvalid && (g[i] < p.dimD[i]);
-        }
-        rvalid = rvalid && tile_ok;
-        grow = ((static_cast<long>(g[3]) * p.dimD[2] + g[2]) * p.dimD[1] + g[1]) * p.dimD[0] + g[0];
-      }
-      const int n0 = nt * OUT_BN;
-      const float* bias2row = ((HAS_BIAS2 || DIRECT) && p.bias2 != nullptr && rvalid)
-                                  ? p.bias2 + (grow / p.rows_per_bias2) * static_cast<long>(p.ld_bias2)
-                                  : nullptr;
-      const uint8_t* resrow = ((HAS_RES || DIRECT) && p.residual != nullptr && rvalid)
-                                  ? reinterpret_cast<const uint8_t*>(p.residual) + grow * p.ld_res * 2
-                                  : nullptr;
-      if (do_prefetch) prefetch_res_tile(static_cast<long>(tile) + gridDim.x);
-      // residual piece of this thread for the group's FIRST chunk of the tile: it does not depend on the accumulator, so
-      // it is requested before the wait for the main loop and its (DRAM/L2) latency -- ~2 K clk of a ~3 K clk chunk in
-      // the K=320 timelines (profiles/r01_igemm_smallk_timeline_res.log) -- hides behind that wait
-      uint4 rres[HAS_RES ? 4 : 1];
-      if (HAS_RES && resrow != nullptr && n0 + eg * 32 < p.n_out) {
-        const uint4* rp = reinterpret_cast<const uint4*>(resrow + (n0 + eg * 32) * 2);
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) rres[j4] = __ldg(rp + j4);
-      }
-
-      w_tfull.wait(&tfull_bar[as], aph);
-      tc_fence_after();
-#ifdef AAB_IGEMM_TRACE
-      if (p.dbg && blockIdx.x == 0 && leader && tl < 32) p.dbg[16 + 288 + eg * 64 + 2 * tl] = static_cast<unsigned long long>(clock64());
-#endif
-      const uint32_t tmem_acc = tmem_base + as * BN + (static_cast<uint32_t>(q * 32) << 16);
-      bool released = false;
-
-#pragma unroll 1
-      for (int ci = eg; ci < CPT; ci += NUM_EPI_GROUPS) {
-        const int cc = ci * 32;
-        const int col = n0 + cc;                  // global output column of this 32-wide chunk
-        if (col >= p.n_out) break;                // warp-uniform; later chunks of this group are out of range too
-        const long long tm0 = p.dbg ? clock64() : 0;
-        if (HAS_RES && resrow != nullptr && ci != eg) {     // later chunks of the tile: requested here (L2-prefetched)
-          const uint4* rp = reinterpret_cast<const uint4*>(resrow + col * 2);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) rres[j4] = __ldg(rp + j4);
-        }
-        const bool last_read = (ci + NUM_EPI_GROUPS >= CPT || col + 32 * NUM_EPI_GROUPS >= p.n_out);
-        uint4 o[4];                               // the chunk's 32 outputs of this row, packed to 16 bits
-        float v[GEGLU ? 1 : 32];
+      for (int h = 0; h < 2; ++h) {
+        float x[2] = {acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]};
         if (GEGLU) {
-          // value and gate columns in two 16-column halves: 32 live accumulator registers instead of 64 (the 64-register
-          // version spilled inside this loop: 1.07 M local loads per launch, profiles/r01_ncu_full_summaries.md)
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint32_t rv[16], rg[16];
-            tmem_ld_32x16(tmem_acc + cc + hf * 16, rv);
-            tmem_ld_32x16(tmem_acc + BN / 2 + cc + hf * 16, rg);
-            tmem_ld_wait();
-            if (hf == 1 && last_read) {
-              tc_fence_before();
-              if (PAIR) {
-                __syncwarp();
-                if (lane_id() == 0) mbar_arrive_leader(&tempty_bar[as]);
-              } else {
-                mbar_arrive(&tempty_bar[as]);
-              }
-              released = true;
-            }
-            float vv[16], gg[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              vv[j] = __uint_as_float(rv[j]);
-              gg[j] = __uint_as_float(rg[j]);
-            }
+          float g[2] = {acc[4 * (jj + BN / 16) + 2 * h], acc[4 * (jj + BN / 16) + 2 * h + 1]};
+          if (col < p.n_out) {
             if (p.bias != nullptr) {
-              const float4* bp = reinterpret_cast<const float4*>(p.bias + col + hf * 16);
-              const float4* gp = reinterpret_cast<const float4*>(p.bias + p.N / 2 + col + hf * 16);
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                const float4 b = __ldg(bp + j4);
-                const float4 g = __ldg(gp + j4);
-                vv[j4 * 4 + 0] += b.x; vv[j4 * 4 + 1] += b.y; vv[j4 * 4 + 2] += b.z; vv[j4 * 4 + 3] += b.w;
-                gg[j4 * 4 + 0] += g.x; gg[j4 * 4 + 1] += g.y; gg[j4 * 4 + 2] += g.z; gg[j4 * 4 + 3] += g.w;
-              }
+              const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
+              x[0] += bv.x; x[1] += bv.y;
+              g[0] += bg.x; g[1] += bg.y;
             }
-#pragma unroll
-            for (int j = 0; j < 16; ++j) vv[j] *= gelu_fast_f(gg[j]);
-#pragma unroll
-            for (int j4 = 0; j4 < 2; ++j4) {
-              o[hf * 2 + j4].x = pack2(vv[j4 * 8 + 0], vv[j4 * 8 + 1], bf16);
-              o[hf * 2 + j4].y = pack2(vv[j4 * 8 + 2], vv[j4 * 8 + 3], bf16);
-              o[hf * 2 + j4].z = pack2(vv[j4 * 8 + 4], vv[j4 * 8 + 5], bf16);
-              o[hf * 2 + j4].w = pack2(vv[j4 * 8 + 6], vv[j4 * 8 + 7], bf16);
+            if (rvalid[h]) {
+              const uint32_t o = pack2(x[0] * gelu_fast_f(g[0]), x[1] * gelu_fast_f(g[1]), bf16);
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(p.out) + (grow[h] * p.ld_out + col) * 2) = o;
+            }
+          }
+        } else if (!direct) {
+          if (col < p.n_out) {
+            if (p.bias != nullptr) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              x[0] += b.x; x[1] += b.y;
+            }
+            if (bias2row[h] != nullptr) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(bias2row[h] + col));
+              x[0] += b.x; x[1] += b.y;
+            }
+            if (resrow[h] != nullptr) {
+              const float2 r = unpack2(__ldg(reinterpret_cast<const unsigned int*>(resrow[h] + col * 2)), bf16);
+              x[0] += r.x; x[1] += r.y;
+            }
+            if (p.act == AAB_ACT_SILU) {
+              x[0] = silu_fast_f(x[0]);
+              x[1] = silu_fast_f(x[1]);
+            }
+            const uint32_t o = pack2(x[0], x[1], bf16);
+            if (rvalid[h]) {
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(p.out) + (grow[h] * p.ld_out + col) * 2) = o;
+              if (stats) {
+                const float2 f = unpack2(o, bf16);           // statistics of the ROUNDED 16-bit outputs
+                ssum[0] += f.x; ssq[0] = fmaf(f.x, f.x, ssq[0]);
+                ssum[1] += f.y; ssq[1] = fmaf(f.y, f.y, ssq[1]);
+              }
             }
           }
         } else {
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_acc + cc, r);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          if (last_read) {
-            // last TMEM read of this group for this tile: give the accumulator stage back before the (slower) store path
-            tc_fence_before();
-            if (PAIR) {
-              __syncwarp();
-              if (lane_id() == 0) mbar_arrive_leader(&tempty_bar[as]);
-            } else {
-              mbar_arrive(&tempty_bar[as]);
-            }
-            released = true;
-          }
-        }
-        if (!DIRECT) {
-          // ---------------- fast path: n_out % 32 == 0, everything vectorised
-          if (!GEGLU) {
-            if (p.bias != nullptr) {
-              const float4* bp = reinterpret_cast<const float4*>(p.bias + col);
-#pragma unroll
-              for (int j4 = 0; j4 < 8; ++j4) {
-                const float4 b = __ldg(bp + j4);
-                v[j4 * 4 + 0] += b.x; v[j4 * 4 + 1] += b.y; v[j4 * 4 + 2] += b.z; v[j4 * 4 + 3] += b.w;
-              }
-            }
-            if (HAS_BIAS2 && bias2row != nullptr) {
-              const float4* bp = reinterpret_cast<const float4*>(bias2row + col);
-#pragma unroll
-              for (int j4 = 0; j4 < 8; ++j4) {
-                const float4 b = __ldg(bp + j4);
-                v[j4 * 4 + 0] += b.x; v[j4 * 4 + 1] += b.y; v[j4 * 4 + 2] += b.z; v[j4 * 4 + 3] += b.w;
-              }
-            }
-            if (HAS_RES && resrow != nullptr) {
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                const uint32_t w[4] = {rres[j4].x, rres[j4].y, rres[j4].z, rres[j4].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = unpack2(w[e], bf16);
-                  v[j4 * 8 + e * 2] += f.x;
-                  v[j4 * 8 + e * 2 + 1] += f.y;
-                }
-              }
-            }
-            if (HAS_SILU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = silu_fast_f(v[j]);
-            }
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              o[j4].x = pack2(v[j4 * 8 + 0], v[j4 * 8 + 1], bf16);
-              o[j4].y = pack2(v[j4 * 8 + 2], v[j4 * 8 + 3], bf16);
-              o[j4].z = pack2(v[j4 * 8 + 4], v[j4 * 8 + 5], bf16);
-              o[j4].w = pack2(v[j4 * 8 + 6], v[j4 * 8 + 7], bf16);
-            }
-          }
-          const long long tm1 = p.dbg ? clock64() : 0;
-          if (!GEGLU && p.colstats != nullptr && !rvalid) {
-            // rows outside the output (partial tiles) are clipped by the TMA store; zeroed here they add nothing to the
-            // column statistics below
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) o[j4] = make_uint4(0, 0, 0, 0);
-          }
-          if (leader) tma_store_wait_read<0>();    // the group's previous store has drained the staging buffer
-          named_bar_sync(bar_id, 128);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) *reinterpret_cast<uint4*>(rowp + ((j4 ^ sw) << 4)) = o[j4];
-          fence_proxy_async_smem();
-          named_bar_sync(bar_id, 128);
-          if (leader && tile_ok) {
-            tma_store_5d(&tmD, stage_buf, col, cb[0], cb[1], cb[2], cb[3]);
-            tma_store_commit();
-          }
-          if (!GEGLU && p.colstats != nullptr) {
-            // GroupNorm statistics of the tensor being written, from the staged (rounded) tile: warp q of the group owns the
-            // 8 columns of 16-byte piece q, lane l the rows l, l+32, l+64, l+96 (conflict-free through the 64B swizzle);
-            // fixed-order butterfly over the lanes -> one (sum, sumsq) pair per column and m-tile, bitwise reproducible.
-            float v[16];                                     // v[j]: sum of column j, v[8 + j]: its sum of squares
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = 0.f;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int r = static_cast<int>(lane_id()) + 32 * i;
-              const uint4 u = *reinterpret_cast<const uint4*>(stage_buf + r * 64 + ((q ^ ((r >> 1) & 3)) << 4));
-              const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 f = unpack2(w[e], bf16);
-                v[2 * e] += f.x; v[8 + 2 * e] = fmaf(f.x, f.x, v[8 + 2 * e]);
-                v[2 * e + 1] += f.y; v[9 + 2 * e] = fmaf(f.y, f.y, v[9 + 2 * e]);
-              }
-            }
-            // reduce-scatter over the lanes (16 shuffles instead of 80): at distance `off` a lane keeps one half of its
-            // values and hands the other half to its partner; afterwards lane l holds the warp total of value
-            // idx = (l>>4 & 1) << 3 | (l>>3 & 1) << 2 | (l>>2 & 1) << 1 | (l>>1 & 1)
-#pragma unroll
-            for (int half = 8; half >= 1; half >>= 1) {
-              const int off = half * 2;
-              const bool up = (lane_id() & off) != 0;
-#pragma unroll
-              for (int jj = 0; jj < half; ++jj) {
-                const float send = up ? v[jj] : v[jj + half];
-                const float keep = up ? v[jj + half] : v[jj];
-                v[jj] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-              }
-            }
-            v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-            if (!(lane_id() & 1) && tile_ok) {
-              const uint32_t l = lane_id();
-              const uint32_t idx = ((l >> 4) & 1) << 3 | ((l >> 3) & 1) << 2 | ((l >> 2) & 1) << 1 | ((l >> 1) & 1);
-              p.colstats[(static_cast<long>(mt_lin) * p.n_out + col + q * 8 + (idx & 7)) * 2 + (idx >> 3)] = v[0];
-            }
-          }
-          if (p.dbg) {
-            t_math += static_cast<unsigned long long>(tm1 - tm0);
-            t_bar += static_cast<unsigned long long>(clock64() - tm1);
-          }
-        } else {
-          // ---------------- generic path: masked, any n_out, fp32 or 16-bit output, straight to global memory
-          const int nv = (p.n_out - col < 32) ? (p.n_out - col) : 32;
-#pragma unroll 1
-          for (int j = 0; j < 32; ++j) {
-            // v[] is indexed dynamically here on purpose (compact code); it lives in local memory on this path
-            if (j < nv) {
-              float x = v[j];
-              if (p.bias != nullptr) x += __ldg(p.bias + col + j);
-              if (bias2row != nullptr) x += __ldg(bias2row + col + j);
-              if (p.flags & AAB_F_SCALE_ACC) {
-                x = apply_act(x, p.act) * p.out_scale;
-                if (resrow != nullptr) x += load_elem(resrow, col + j, bf16);
+          for (int e = 0; e < 2; ++e) {
+            if (col + e < p.n_out) {
+              float v = x[e];
+              if (p.bias != nullptr) v += __ldg(p.bias + col + e);
+              if (bias2row[h] != nullptr) v += __ldg(bias2row[h] + col + e);
+              if (scale_acc) {
+                v = apply_act(v, p.act) * p.out_scale;
+                if (resrow[h] != nullptr) v += load_elem(resrow[h], col + e, bf16);
               } else {
-                if (resrow != nullptr) x += load_elem(resrow, col + j, bf16);
-                x = apply_act(x, p.act) * p.out_scale;
+                if (resrow[h] != nullptr) v += load_elem(resrow[h], col + e, bf16);
+                v = apply_act(v, p.act) * p.out_scale;
               }
-              if (rvalid) {
-                if (p.flags & AAB_F_OUT_F32) reinterpret_cast<float*>(p.out)[grow * p.ld_out + col + j] = x;
-                else store_elem(p.out, grow * p.ld_out + col + j, x, bf16);
+              if (rvalid[h]) {
+                if (out_f32) reinterpret_cast<float*>(p.out)[grow[h] * p.ld_out + col + e] = v;
+                else store_elem(p.out, grow[h] * p.ld_out + col + e, v, bf16);
               }
             }
           }
         }
       }
-      if (!released) {                            // this group had no chunk in range for this tile
-        tc_fence_before();
-        if (PAIR) {
-          __syncwarp();
-          if (lane_id() == 0) mbar_arrive_leader(&tempty_bar[as]);
-        } else {
-          mbar_arrive(&tempty_bar[as]);
+      if (stats) {
+        // sum over the warp's 16 rows: the 8 lanes sharing (lane & 3) hold this column pair; fixed-order butterfly
+#pragma unroll
+        for (int off = 4; off < 32; off <<= 1) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            ssum[e] += __shfl_xor_sync(0xffffffffu, ssum[e], off);
+            ssq[e] += __shfl_xor_sync(0xffffffffu, ssq[e], off);
+          }
+        }
+        if (lane < 4) {
+          float* sp = sstats + ((cw * 4 + wq) * BN + cl) * 2;
+          sp[0] = ssum[0]; sp[1] = ssq[0]; sp[2] = ssum[1]; sp[3] = ssq[1];
         }
       }
-#ifdef AAB_IGEMM_TRACE
-      if (p.dbg && blockIdx.x == 0 && leader && tl < 32) p.dbg[16 + 288 + eg * 64 + 2 * tl + 1] = static_cast<unsigned long long>(clock64());
-#endif
     }
-    if (!DIRECT && leader) tma_store_wait_all<0>();
-    if (leader && eg == 0) {
-      w_tfull.flush(p.dbg, 5);                                   // slot 5: epilogue group 0 waiting for the accumulator
-      if (p.dbg) {
-        atomicAdd(p.dbg + 6, t_math);                            // slot 6: residual/TMEM load + math + pack (group 0)
-        atomicAdd(p.dbg + 7, t_bar);                             // slot 7: drain wait + barriers + st.shared + store issue
+    if (stats) {
+      // the eight warps' partial sums, added in warp order -> one (sum, sumsq) pair per column and m-tile, reproducible
+      named_bar_sync(1, 128 * NUM_CONSUMERS);
+      for (int c = static_cast<int>(threadIdx.x) - 128; c < OUT_BN && tile_ok; c += 128 * NUM_CONSUMERS) {
+        if (n0 + c >= p.n_out) break;
+        float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int w = 0; w < NUM_CONSUMER_WARPS; ++w) {
+          s0 += sstats[(w * BN + c) * 2];
+          s1 += sstats[(w * BN + c) * 2 + 1];
+        }
+        p.colstats[(static_cast<long>(mt_lin) * p.n_out + n0 + c) * 2] = s0;
+        p.colstats[(static_cast<long>(mt_lin) * p.n_out + n0 + c) * 2 + 1] = s1;
       }
     }
   }
-
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();     // neither CTA may exit (or free TMEM) while the peer can still signal into it
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
-    else tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
+  if (CL > 1) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -693,89 +410,78 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
 
-template <int BN, int EPI>
-static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const CUtensorMap& d,
-                     const CUtensorMap& r, const IgemmParams& p, int max_ctas, cudaStream_t stream) {
+template <int BN, bool GEGLU, bool BF16>
+static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
+                    int max_ctas, cudaStream_t stream) {
   using CF = Cfg<BN>;
   static std::atomic<unsigned long long> attr_done{0};
-  if (int r = ensure_dyn_smem(igemm_kernel<BN, EPI>, CF::SMEM_BYTES, attr_done)) return r;
-  int tiles = p.num_m_tiles * p.num_n_tiles;
-  int grid = tiles < num_sms() ? tiles : num_sms();
-  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  launch_k(igemm_kernel<BN, EPI>, dim3(grid), dim3(NUM_THREADS), CF::SMEM_BYTES, stream, a, a2, b, d, r, p);
-  return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
-}
-
-// CTA-pair launch: clusters of 2 (or 4: p.cluster), persistent over cluster tiles (p.cluster consecutive m-tiles x one n-tile)
-template <int EPI>
-static int launch_pair(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const CUtensorMap& d,
-                       const CUtensorMap& r, const IgemmParams& p, int max_ctas, cudaStream_t stream) {
-  using CF = Cfg<256, true>;
-  static std::atomic<unsigned long long> attr_done{0};
-  if (int rc = ensure_dyn_smem(igemm_kernel<256, EPI, true>, CF::SMEM_BYTES, attr_done)) return rc;
+  if (int r = ensure_dyn_smem(igemm_kernel<BN, GEGLU, BF16>, CF::SMEM_BYTES, attr_done)) return r;
   const int cl = p.cluster;
-  const int cl_tiles = ((p.num_m_tiles + cl - 1) / cl) * p.num_n_tiles;
+  const int tiles = ((p.num_m_tiles + cl - 1) / cl) * p.num_n_tiles;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(NUM_THREADS);
   cfg.dynamicSmemBytes = CF::SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = static_cast<unsigned>(cl);
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  int na = 0;
+  if (cl > 1) {
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = static_cast<unsigned>(cl);
+    attr[na].val.clusterDim.y = 1;
+    attr[na].val.clusterDim.z = 1;
+    ++na;
+  }
+  if (pdl_enabled()) {
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = na;
   int clusters = num_sms() / cl;
-  if (cl == 4) {
-    // clusters of 4 must fit inside a GPC: ask the driver how many can be resident at once (cached per device)
-    static std::atomic<int> max_quads[64];
+  if (cl > 1) {
+    // a cluster's CTAs must fit inside one GPC: ask the driver how many clusters can be resident at once (cached per device)
+    static std::atomic<int> max_clusters[64];
     int dev = 0;
     cudaGetDevice(&dev);
-    int mq = max_quads[dev & 63].load(std::memory_order_acquire);
-    if (mq == 0) {
-      cfg.gridDim = dim3(static_cast<unsigned>(4 * (num_sms() / 4)));
+    int mc = max_clusters[dev & 63].load(std::memory_order_acquire);
+    if (mc == 0) {
+      cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<256, EPI, true>, &cfg) != cudaSuccess || n < 1) {
+      if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<BN, GEGLU, BF16>, &cfg) != cudaSuccess || n < 1) {
         cudaGetLastError();
         n = 1;
       }
-      mq = n;
-      max_quads[dev & 63].store(mq, std::memory_order_release);
+      mc = n;
+      max_clusters[dev & 63].store(mc, std::memory_order_release);
     }
-    if (clusters > mq) clusters = mq;
+    if (clusters > mc) clusters = mc;
   }
-  if (cl_tiles < clusters) clusters = cl_tiles;
+  if (tiles < clusters) clusters = tiles;
   if (max_ctas > 0 && clusters > max_ctas / cl) clusters = max_ctas / cl > 0 ? max_ctas / cl : 1;
   cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, igemm_kernel<256, EPI, true>, a, a2, b, d, r, p);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, igemm_kernel<BN, GEGLU, BF16>, a, a2, b, p);
   return e == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
 
-template <int EPI>
-static int launch_epi(int bn, const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const CUtensorMap& d,
-                      const CUtensorMap& r, const IgemmParams& p, int max_ctas, cudaStream_t stream) {
-  switch (bn) {
-    case 64: return launch_bn<64, EPI>(a, a2, b, d, r, p, max_ctas, stream);
-    case 128: return launch_bn<128, EPI>(a, a2, b, d, r, p, max_ctas, stream);
-    default: return launch_bn<256, EPI>(a, a2, b, d, r, p, max_ctas, stream);
-  }
+template <int BN, bool GEGLU>
+static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
+                     int max_ctas, cudaStream_t stream) {
+  if (p.flags & AAB_F_BF16) return launch_t<BN, GEGLU, true>(a, a2, b, p, max_ctas, stream);
+  return launch_t<BN, GEGLU, false>(a, a2, b, p, max_ctas, stream);
 }
 
 }  // namespace aab
 
 using namespace aab;
 
-// 1 when this launch takes a staged (smem + TMA store) epilogue -- the only ones that can emit `colstats` -- else 0
+// 1 when this launch takes a staged epilogue -- the only ones that can emit `colstats` -- else 0
 static int igemm_is_staged(const AabIgemmDesc* d) {
   const bool geglu = (d->flags & AAB_F_GEGLU) != 0;
   const int bn = d->block_n;
@@ -802,11 +508,11 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
   bool direct = (d->flags & AAB_F_DIRECT) != 0;
   const int n_out = geglu ? d->n / 2 : d->n;
   if (bn == 32 || (d->ld_out % 8) != 0 || (n_out % 32) != 0 || (d->flags & AAB_F_OUT_F32)) direct = true;
-  if (geglu && (bn < 128 || direct)) return AAB_ERR_ARG;   // output tile must cover whole 64-column store boxes
+  if (geglu && (bn < 128 || direct)) return AAB_ERR_ARG;   // the gate half of the tile must be a whole number of 64-column blocks
   if (d->residual && (d->ld_res % 8) != 0 && !direct) direct = true;
   if (d->flags & AAB_F_SCALE_ACC) direct = true;
   if ((d->act == AAB_ACT_GELU || d->act == AAB_ACT_QUICK_GELU) && !geglu) direct = true;
-  {   // the staged variants cover one extra term each (residual | per-sample bias | SiLU) and no output scaling
+  {   // the staged epilogue covers one extra term (residual | per-sample bias | SiLU) and no output scaling
     const int extras = (d->residual ? 1 : 0) + (d->bias2 ? 1 : 0) + (d->act == AAB_ACT_SILU ? 1 : 0);
     if (!geglu && (extras > 1 || d->out_scale != 1.0f)) direct = true;
     if (geglu && (extras > 0 || d->out_scale != 1.0f)) return AAB_ERR_ARG;
@@ -850,10 +556,9 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
   p.out_scale = d->out_scale;
   p.act = d->act;
   p.flags = d->flags | (direct ? AAB_F_DIRECT : 0);
-  p.dbg = d->debug_cycles;
   p.colstats = direct ? nullptr : d->colstats;   // staged epilogues only (the caller checks the result of aab_igemm_emits_colstats)
 
-  CUtensorMap tmA, tmA2, tmB, tmD, tmR;
+  CUtensorMap tmA, tmA2, tmB;
   {
     int box[5] = {BK, d->box[0], d->box[1], d->box[2], d->box[3]};
     int r = make_tmap_16(&tmA, d->a, 5, d->a_dims, d->a_strides, box, is_bf16, 128);
@@ -865,67 +570,27 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
       tmA2 = tmA;
     }
   }
+  // clusters sharing each weight tile: 256-column staged tiles with unbatched weights and at least two m-tiles
+  const bool pair = (d->flags & AAB_F_PAIR) != 0 && bn == 256 && !direct && d->b_batch_dim < 0 && p.num_m_tiles >= 2;
+  p.cluster = pair ? (((d->flags & AAB_F_QUAD) && p.num_m_tiles >= 4) ? 4 : 2) : 1;
   {
     long dims[3] = {static_cast<long>(d->num_taps) * d->kc, d->n, d->b_batch > 0 ? d->b_batch : 1};
     long strides[3] = {1, d->ld_b, d->b_batch_stride > 0 ? d->b_batch_stride : static_cast<long>(d->n) * d->ld_b};
-    int box[3] = {BK, geglu ? bn / 2 : bn, 1};
+    const int slices = p.cluster > 1 ? p.cluster : (geglu ? 2 : 1);   // rows of one weight-tile slice (see the producer)
+    int box[3] = {BK, bn / slices, 1};
     int r = make_tmap_16(&tmB, d->b, 3, dims, strides, box, is_bf16, 128);
     if (r) return r;
   }
-  if (!direct) {
-    // D (and the residual) viewed with the same pixel decomposition as the tile grid: [n_out, dimD0..3]; rows are
-    // contiguous in pixel-linear order with a row stride of ld_out (ld_res) elements.  32-column boxes, 64B swizzle.
-    long dims[5] = {n_out, d->dim_d[0], d->dim_d[1], d->dim_d[2], d->dim_d[3]};
-    long strides[5];
-    strides[0] = 1;
-    strides[1] = d->ld_out;
-    for (int i = 2; i < 5; ++i) strides[i] = strides[i - 1] * d->dim_d[i - 2];
-    int box[5] = {32, d->box[0], d->box[1], d->box[2], d->box[3]};
-    int r = make_tmap_16(&tmD, d->out, 5, dims, strides, box, is_bf16, 64);
-    if (r) return r;
-    if (d->residual) {
-      strides[1] = d->ld_res;
-      for (int i = 2; i < 5; ++i) strides[i] = strides[i - 1] * d->dim_d[i - 2];
-      r = make_tmap_16(&tmR, d->residual, 5, dims, strides, box, is_bf16, 64);
-      if (r) return r;
-    } else {
-      tmR = tmD;
-    }
-  } else {
-    tmD = tmB;
-    tmR = tmB;
-  }
-  // CTA pairs (cta_group::2): 256-column tiles of the staged epilogues; the tile box of B is half a tile per CTA
-  const bool pair = (d->flags & AAB_F_PAIR) != 0 && bn == 256 && !direct && d->b_batch_dim < 0 && p.num_m_tiles >= 2;
-  if (pair) {
-    long dimsb[3] = {static_cast<long>(d->num_taps) * d->kc, d->n, 1};
-    long stridesb[3] = {1, d->ld_b, static_cast<long>(d->n) * d->ld_b};
-    p.cluster = ((d->flags & AAB_F_QUAD) && p.num_m_tiles >= 4) ? 4 : 2;
-    int boxb[3] = {BK, p.cluster == 4 ? 64 : 128, 1};      // QUAD: every CTA fetches a quarter of the weight tile
-    int rb = make_tmap_16(&tmB, d->b, 3, dimsb, stridesb, boxb, is_bf16, 128);
-    if (rb) return rb;
-    if (geglu) return launch_pair<1>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    if (d->residual) return launch_pair<3>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    if (d->bias2) return launch_pair<4>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    if (d->act == AAB_ACT_SILU) return launch_pair<5>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    return launch_pair<0>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-  }
-  if (direct) {
-    switch (bn) {
-      case 32: return launch_bn<32, 2>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-      case 64: return launch_bn<64, 2>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-      case 128: return launch_bn<128, 2>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-      default: return launch_bn<256, 2>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    }
-  }
   if (geglu) {
-    if (bn == 128) return launch_bn<128, 1>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-    return launch_bn<256, 1>(tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
+    if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    return launch_bn<256, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);
   }
-  if (d->residual) return launch_epi<3>(bn, tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-  if (d->bias2) return launch_epi<4>(bn, tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-  if (d->act == AAB_ACT_SILU) return launch_epi<5>(bn, tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
-  return launch_epi<0>(bn, tmA, tmA2, tmB, tmD, tmR, p, d->max_ctas, stream);
+  switch (bn) {
+    case 32: return launch_bn<32, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    case 64: return launch_bn<64, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    case 128: return launch_bn<128, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    default: return launch_bn<256, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+  }
 }
 
 extern "C" int aab_num_sms(void) { return aab::num_sms(); }

@@ -10,16 +10,12 @@
 #define AAB_ACT_QUICK_GELU 3   /* x * sigmoid(1.702 x): transformers 'quick_gelu' (CLIP text MLP) */
 
 #define AAB_F_BF16 1      /* 16-bit type is bfloat16 (else float16) */
-#define AAB_F_DIRECT 2    /* epilogue stores straight to global memory instead of smem + TMA store */
+#define AAB_F_DIRECT 2    /* generic epilogue: any n_out, fp32 output, every flag combination, per-element masks */
 #define AAB_F_OUT_F32 4   /* output is float32 (direct store only) */
-#define AAB_F_DBG_NO_MMA 64   /* diagnostics only (wrong results): stages are released without issuing tcgen05.mma -> pure TMA feed rate */
-#define AAB_F_DBG_NO_PEEK 4096 /* diagnostics only: blocking full-barrier wait before every k-block (the pre-peek issue loop) */
-#define AAB_F_DBG_NO_SYNC 256 /* diagnostics only: with NO_LOAD, the MMA warp neither waits for stages nor commits them -> raw tcgen05.mma issue rate */
-#define AAB_F_DBG_NO_LOAD 128 /* diagnostics only (wrong results): no TMA loads, stages are always full -> pure MMA + epilogue rate */
 #define AAB_F_SCALE_ACC 16 /* out = act(acc + bias + bias2) * out_scale + residual (scale BEFORE the residual; direct store only) */
-#define AAB_F_QUAD 16384 /* with AAB_F_PAIR: clusters of 4 = two CTA pairs stacked along M; every weight tile is fetched once per cluster (TMA multicast) */
-#define AAB_F_PAIR 32     /* 256-column tiles on CTA pairs (cta_group::2): two m-tiles per tcgen05.mma, half a weight tile per CTA */
 #define AAB_F_GEGLU 8     /* B rows [0,N/2) are values, [N/2,N) gates: out = value * gelu(gate), N/2 columns */
+#define AAB_F_PAIR 32     /* 256-column staged tiles on clusters of two CTAs sharing each weight tile (TMA multicast) */
+#define AAB_F_QUAD 16384  /* with AAB_F_PAIR: clusters of four (launches with fewer than 4 m-tiles use clusters of two) */
 
 #ifdef __cplusplus
 extern "C" {
@@ -58,10 +54,9 @@ typedef struct AabIgemmDesc {
   int flags;
   int block_n;              // 32 / 64 / 128 / 256
   int max_ctas;             // 0 = one CTA per SM
-  unsigned long long* debug_cycles;   // optional [16] device counters: per-role wait cycles (profiling aid), or NULL
   float* colstats;          // optional [num_m_tiles][n_out][2] fp32: per m-tile column sums (sum, sum of squares) of the ROUNDED
                             // 16-bit outputs over the tile's valid rows -- the statistics of the GroupNorm that follows, taken
-                            // where the data already is in registers / shared memory (staged epilogues only), or NULL
+                            // where the data already is in registers (staged epilogues only), or NULL
 } AabIgemmDesc;
 
 #ifdef __cplusplus
@@ -89,9 +84,8 @@ struct IgemmParams {
   float out_scale;
   int act;
   int flags;
-  unsigned long long* dbg;
   float* colstats;
-  int cluster;     /* CTAs per cluster of the pair kernels: 2, or 4 (two pairs sharing the weight tile through TMA multicast) */
+  int cluster;     /* CTAs per cluster sharing each weight tile: 1, 2 or 4 */
 };
 int make_tmap_16(CUtensorMap* out, const void* base, int rank, const long* dims, const long* strides, const int* box,
                  int is_bf16, int swizzle_bytes = 128);

@@ -365,7 +365,7 @@ layernorm_kernel(const void* __restrict__ x, long ldx, void* __restrict__ y, lon
   }
 }
 
-// LayerNorm v2 (round 2; v1 reached 0.48 of the HBM roofline): LPR lanes share one row (LPR = 8 / 16 / 32 chosen so that
+// LayerNorm v2 (v1 leaves lanes idle for C = 320 / 640): LPR lanes share one row (LPR = 8 / 16 / 32 chosen so that
 // ceil(C/8 / LPR) octets per lane waste no lanes: C=320 -> 8 lanes x 5 octets, 640 -> 16 x 5, 1280 -> 32 x 5), a warp
 // normalises 32/LPR rows at once, persistent warps walk the row groups and the NEXT group's loads are issued before the
 // current group is reduced (register double buffering), so every warp always has loads in flight.  Exact two-pass
@@ -498,8 +498,7 @@ static int gn_launch_cfg(int C, long samples, long rows, int* threads, int* rows
   *threads = V * rpi;
   // The row partition depends on (rows, C) only -- never on the number of samples -- so a sample's statistics are
   // summed in the same order whatever batch it arrives in (CFG halves split over two GPUs stay bit-identical to the
-  // batched evaluation).  Elements per CTA from the measured sweep (profiles/r01_gn_chunk_sweep.md): 72K for the
-  // wide-row levels (C <= 640, or very large samples), 18K where C >= 1280 (few rows per sample: CTA count matters),
+  // batched evaluation).  Elements per CTA: 72K for the wide-row levels (C <= 640, or very large samples), 18K where C >= 1280 (few rows per sample: CTA count matters),
   // 12K for tiny samples; at least 8 row-iterations per CTA; at most 1024 chunks per sample.
   (void)samples;
   const long elems = rows * C;
@@ -516,9 +515,8 @@ static int gn_launch_cfg(int C, long samples, long rows, int* threads, int* rows
 }
 
 // The apply pass is elementwise: its row partition is free (unlike the statistics pass, whose partition fixes the summation
-// order).  The statistics partition gives 612 CTAs at level 0 = 1.38 waves of the 444 resident CTAs (3 per SM): the second wave
-// runs 38 % full.  Here the rows are cut so that the launch is ~3 waves of CTAs (AAB_GN_APPLY_WAVES; measured 0 / 3 / 6 / 12: 73.4 / 70.7 / 73.5 / 79.7 us at level 0; 0 = the statistics
-// partition), each thread still walking >= 4 rows.
+// order).  The statistics partition can leave a partly filled last wave of CTAs; here the rows are cut so that the launch is
+// ~3 waves of CTAs (AAB_GN_APPLY_WAVES; 0 = the statistics partition), each thread still walking >= 4 rows.
 static int gn_apply_rows_per_cta(int C, long samples, long rows, int stats_rpc) {
   static int waves = -1;
   if (waves < 0) {
@@ -580,10 +578,8 @@ extern "C" int aab_groupnorm(const void* x1, long ld1, int c1, const void* x2, l
   const size_t smem_red = static_cast<size_t>(threads / groups) * groups * 2 * sizeof(double);
   if (smem_red > smem) smem = smem_red;
   if (smem > 48 * 1024 || threads < groups) return AAB_ERR_ARG;
-  // A fused single-launch variant (cooperative grid: statistics -> per-sample flag -> apply) was built and measured in
-  // round 2 and LOST to this pair in every shape (profiles/r02_kernel_ab_fusedGN_LNv2_TAv2.md vs ..._round1_kernels.md:
-  // 84 vs 72 us at [34, 4096, 320], 38 vs 24 us at [34, 256, 1280]): the flag wait serialises the two phases inside every
-  // CTA, while two plain launches let the hardware overlap the tail of one with the head of the next.  Not kept.
+  // Two launches rather than one cooperative grid (statistics -> per-sample flag -> apply): a flag wait would serialise the
+  // two phases inside every CTA, while two plain launches let the hardware overlap the tail of one with the head of the next.
   dim3 grid(static_cast<unsigned>(chunks), static_cast<unsigned>(samples));
   launch_k(gn_stats_kernel, dim3(grid), dim3(threads), smem, stream, a, partial, mean_rstd, ticket, eps);
   {

@@ -1,4 +1,4 @@
-"""Executes the parameter containers of `layers.py` on the sm_100a kernels.
+"""Executes the parameter containers of `layers.py` on the sm_90a kernels.
 
 Activation layout: 2-D tensors [rows, C] with rows ordered (batch b, frame t, y, x) — i.e. channels-last
 [B, T, H, W, C].  The reference's `(b t) c h w  <->  b c t h w  <->  (b h w) t c` permutes

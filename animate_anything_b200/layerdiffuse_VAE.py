@@ -1,4 +1,4 @@
-"""B200 mirror of the reference's `models/layerdiffuse_VAE.py` (SURVEY row f4, the transparent-video branch):
+"""Mirror of the reference's `models/layerdiffuse_VAE.py` (SURVEY row f4, the transparent-video branch):
 
   LatentTransparencyOffsetEncoder   :17-41   RGBA image -> latent offset, nine 3x3 convs with SiLU (called once per clip at
                                              train_transparent_i2v_stage2.py:415)
@@ -10,7 +10,7 @@ diffusers 0.24 `get_down_block` / `get_up_block` / `UNetMidBlock2D`: DownBlock2D
 `temb_channels=None`, GroupNorm(4)), so the reference's `vae_alpha_decoder.pth` / `vae_alpha_encoder.pth` load unchanged.
 
 Everything runs on the kernels of the denoising path — no new GEMM or attention kernel:
-  * every convolution (3x3, stride 2, 1x1) on the tcgen05 implicit GEMM; SiLU of the encoder in the GEMM epilogue;
+  * every convolution (3x3, stride 2, 1x1) on the wgmma implicit GEMM; SiLU of the encoder in the GEMM epilogue;
     32-channel tensors in front of a stride-2 conv are widened to the 64-channel K block (`aab_pad_cols`), skip concats
     are virtual except where the first source is narrower than one K block (32 channels: one strided copy);
   * GroupNorm(4)+SiLU on the GroupNorm kernels (statistics from the producing GEMM where the tile geometry allows);
@@ -70,7 +70,7 @@ class LatentTransparencyOffsetEncoder(ModelBase):
         if prep is not None and prep.dtype == p0.dtype and prep.device == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16) or not p0.is_cuda:
-            raise TypeError("LatentTransparencyOffsetEncoder must be fp16/bf16 on a CUDA device for the sm_100a path (no fallback)")
+            raise TypeError("LatentTransparencyOffsetEncoder must be fp16/bf16 on a CUDA device for the sm_90a path (no fallback)")
         prep = self._build_prepared(p0.dtype, p0.device)
         self.__dict__["_aab_prepared"] = prep
         return prep
@@ -246,7 +246,7 @@ class UNet384(ModelBase):
         if prep is not None and prep.dtype == p0.dtype and prep.device == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16) or not p0.is_cuda:
-            raise TypeError("UNet384 must be fp16/bf16 on a CUDA device for the sm_100a path (no fallback)")
+            raise TypeError("UNet384 must be fp16/bf16 on a CUDA device for the sm_90a path (no fallback)")
         prep = self._build_prepared(p0.dtype, p0.device)
         self.__dict__["_aab_prepared"] = prep
         return prep

@@ -2,7 +2,7 @@
 (models/unet_3d_blocks.py:18-20, models/unet_3d_condition_mask.py:24-26).  Same attribute names, hence the same
 `state_dict()` keys as the reference checkpoints (utils/convert_diffusers_to_original_ms_text_to_video.py:18-169).
 
-These classes hold parameters only.  They deliberately have no torch `forward`: all arithmetic runs in the sm_100a
+These classes hold parameters only.  They deliberately have no torch `forward`: all arithmetic runs in the sm_90a
 kernels driven by `engine.py`; calling them directly raises, so a silent eager fallback cannot happen.
 """
 from __future__ import annotations
@@ -13,7 +13,7 @@ import torch.nn as nn
 
 class _ParamsOnly(nn.Module):
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError(f"{type(self).__name__} is a parameter container; the B200 engine executes it "
+        raise RuntimeError(f"{type(self).__name__} is a parameter container; the sm_90a engine executes it "
                            f"(animate_anything_b200.engine). There is no eager fallback.")
 
 

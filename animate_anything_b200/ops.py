@@ -1,5 +1,5 @@
 """Tensor-level wrappers over the C-ABI (`_lib.call`).  Activations are channels-last 16-bit torch tensors; torch only
-provides memory and the current stream.  Every function here launches hand-written sm_100a kernels — nothing falls back
+provides memory and the current stream.  Every function here launches hand-written sm_90a kernels — nothing falls back
 to torch compute.
 """
 from __future__ import annotations
@@ -15,18 +15,17 @@ from . import _lib
 from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, F_BF16, F_DIRECT, F_GEGLU, F_OUT_F32, F_PAIR, F_QUAD, F_SCALE_ACC,
                    IgemmDesc)
 
-NUM_SMS = 148
-IGEMM_DEBUG = None       # optional uint64[16] device tensor: per-role wait-cycle counters (tools/igemm_roles.py)
-IGEMM_DBG_FLAGS = 4096 if os.environ.get("AAB_IGEMM_NOPEEK") else 0     # tools/igemm_roles.py only: AAB_F_DBG_NO_MMA (64) / AAB_F_DBG_NO_LOAD (128); results are wrong by design
+NUM_SMS = 132           # H100 SXM
 IGEMM_PROFILE = None     # bench.py sets this to a list to time every implicit-GEMM launch with CUDA events
-# 256-column tiles on CTA pairs (cta_group::2).  AAB_IGEMM_PAIR=0 restores the single-CTA kernel everywhere, =2 forces pairs
-# wherever the kernel supports them (A/B runs); default: pairs where they won in profiles/r02_igemm_pair_vs_single.md.
-IGEMM_PAIR = {"0": False, "2": "all"}.get(os.environ.get("AAB_IGEMM_PAIR", "1"), True)
+# 256-column tiles on clusters of two CTAs that share each weight tile through TMA multicast.  Off by default: on an H100 SXM
+# at a 400 W power limit the config-2 UNet forward's GEMMs took 264 ms with clusters on the long-K launches against 199 ms
+# on single CTAs (same call, bench.py).  AAB_IGEMM_PAIR=1 enables them where use_pair says, =2 wherever the kernel supports them.
+IGEMM_PAIR = {"0": False, "2": "all"}.get(os.environ.get("AAB_IGEMM_PAIR", "0"), True)
 
 
 def use_pair(k_total: int, n: int) -> bool:
-    """Pairs pay where the main loop dominates (measured on every launch shape of a config-2 forward: +10-24 % for K >= 960,
-    and for K >= 512 with wide outputs); short K loops (K <= 640 with N <= 1280) are epilogue / latency bound and lose."""
+    """Clusters pay where the main loop dominates and the weight tile is re-read by many m-tiles: long K (>= 960), or
+    K >= 512 with wide outputs; short-K launches are epilogue / latency bound."""
     if IGEMM_PAIR == "all":
         return True
     return bool(IGEMM_PAIR) and (k_total >= 960 or (k_total >= 512 and n >= 1536))
@@ -99,27 +98,26 @@ def _tiles_cover_rows_in_order(dim_d, box) -> bool:
     return all(box[j] == 1 for j in range(i, 4))
 
 
-IGEMM_QUAD = os.environ.get("AAB_IGEMM_QUAD", "0") != "0"     # clusters of 4 with weight-tile multicast (see igemm.cu)
+IGEMM_QUAD = os.environ.get("AAB_IGEMM_QUAD", "0") != "0"     # clusters of four instead of two (see igemm.cu)
 GN_COLSTATS = os.environ.get("AAB_GN_COLSTATS", "1") != "0"
 N64_NARROW = os.environ.get("AAB_IGEMM_N64_NARROW", "1") != "0"
 
 
 def pick_block_n(n_out: int, m_tiles: int, geglu: bool = False, k_total: int = 1 << 30) -> int:
-    """Tile width (GEMM columns, multiple of 32, <= 256).  Measured (profiles/r01_igemm_roles_small.log): a k-block
-    costs ~520-660 clk whatever the tile width (operand feed, not MMA rate), so the widest tile wins wherever the main
-    loop dominates -- even when it leaves SMs without a tile (8x8 level: 85 tiles of 256 beat 170 tiles of 128 by 1.7x).
-    A ragged last N tile costs neither MMA cycles (per-tile UMMA N) nor traffic (TMA zero-fill)."""
+    """Tile width (GEMM columns, multiple of 32, <= 256).  The widest tile wins wherever the main loop dominates: every
+    k-block loads the same 16 KiB of activations whatever the width, so a wide tile reads A once for more columns.  A ragged
+    last N tile costs no traffic (TMA zero-fill beyond N)."""
     if geglu:
         return 256 if n_out > 64 else 128
     if m_tiles <= 2:
         return 64           # weight-streaming (GEMV-like: text K/V, time embedding): spread the weight rows over many CTAs
     if n_out <= 64 and N64_NARROW:
-        # a 64-column output on a 256-column tile stages 32 KiB of (mostly zero-filled) weight rows per k-block and leaves
-        # room for one CTA per SM; UNet384's 64-channel levels (1-4 M rows) are HBM / latency bound and want the narrow tile
-        # (A/B: profiles/r02c_alpha_tail_kernels_*.md).  No shape of the SD UNet / VAE / SVD / CLIP paths has N <= 64.
+        # a 64-column output on a 256-column tile computes and stages mostly zero-filled weight rows; UNet384's 64-channel
+        # levels (1-4 M rows) are HBM / latency bound and want the narrow tile.  No shape of the SD UNet / VAE / SVD / CLIP
+        # paths has N <= 64.
         return 64
     if k_total <= 384 and n_out <= 640:
-        # epilogue/HBM-bound (tiny K): more CTAs in flight hide the store drain; BN=128 has 6 stages, BN=64 has 8
+        # epilogue/HBM-bound (tiny K): more tiles than SMs keep every SM busy
         return 128 if m_tiles * -(-n_out // 128) >= NUM_SMS else 64
     return 256
 
@@ -205,13 +203,10 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
     d.act = act
     flags = ((F_BF16 if bf else 0) | (F_GEGLU if geglu else 0) | (F_OUT_F32 if out_f32 else 0) | (F_DIRECT if direct else 0) |
              (F_SCALE_ACC if scale_acc else 0))
-    d.flags = flags | IGEMM_DBG_FLAGS
     if block_n is None:
         if n_out < 64 and not geglu:
-            # 32-column tiles only have the direct-store epilogue (measured on UNet384's 32-channel level, 4.2 M rows:
-            # 2.1-2.4 ms per launch whatever K, profiles/r02c_alpha_tail_kernels_before.md); an output that qualifies for
-            # the staged epilogue (TMA store in 32-column boxes) takes a 64-column tile whose upper half is a ragged,
-            # zero-filled N remainder instead
+            # 32-column tiles only have the direct-store epilogue; an output that qualifies for the staged epilogue (and
+            # its column statistics) takes a 64-column tile whose upper half is a ragged, zero-filled N remainder instead
             staged_ok = (n_out % 32 == 0 and not out_f32 and not direct and not scale_acc and ld_out % 8 == 0 and
                          os.environ.get("AAB_IGEMM_N32_DIRECT", "0") == "0")
             block_n = 64 if (n_out > 32 or staged_ok) else 32
@@ -221,10 +216,9 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         flags |= F_PAIR
         if IGEMM_QUAD:
             flags |= F_QUAD
-    d.flags = flags | IGEMM_DBG_FLAGS
+    d.flags = flags
     d.block_n = block_n
     d.max_ctas = max_ctas
-    d.debug_cycles = None if IGEMM_DEBUG is None else IGEMM_DEBUG.data_ptr()
     cstats = None
     if stats and GN_COLSTATS and not geglu and _tiles_cover_rows_in_order(dim_d, box):
         d.colstats = 1          # placeholder so that the C-side predicate sees "requested"

@@ -1,4 +1,4 @@
-"""B200 mirror of the reference's `models/pipeline.py` `LatentToVideoPipeline.__call__` (:14-214): same keyword
+"""Mirror of the reference's `models/pipeline.py` `LatentToVideoPipeline.__call__` (:14-214): same keyword
 arguments, same return values (`return_dict=False` -> `(video, latents)`), same semantics — classifier-free guidance with
 cat([negative, positive]) embeddings (:136,:161,:165), caller-supplied truncated `timesteps` (:149-152), motion value
 (:167-168), CFG combine (:180-181), scheduler step on `(b f) c h w` (:184-192), VAE decode (:200), tensor2vid (:205).
@@ -97,7 +97,7 @@ class LatentToVideoPipeline:
             raise ValueError("`prompt_embeds` and `negative_prompt_embeds` must have the same shape")
 
     def _b200_text_encoder(self):
-        """The text encoder as an sm_100a `clip_text.CLIPTextModel`.  A `transformers.CLIPTextModel` handed in by the
+        """The text encoder as an sm_90a `clip_text.CLIPTextModel`.  A `transformers.CLIPTextModel` handed in by the
         caller (train.py:88,799 does exactly that) is mirrored once (same weights, dtype, device) so that prompt strings
         never run a library GEMM / SDPA; the mirror is rebuilt if the caller swaps or moves the encoder."""
         from .clip_text import CLIPTextModel
@@ -117,7 +117,7 @@ class LatentToVideoPipeline:
     def _encode_prompt(self, prompt, device, num_images_per_prompt, do_cfg, negative_prompt=None, prompt_embeds=None,
                        negative_prompt_embeds=None, lora_scale=None):
         """diffusers TextToVideoSDPipeline._encode_prompt: CLIP text states; under CFG returns cat([negative, positive]).
-        The CLIP forward runs on the sm_100a kernels (clip_text.py)."""
+        The CLIP forward runs on the sm_90a kernels (clip_text.py)."""
         def embed(texts):
             if self.text_encoder is None or self.tokenizer is None:
                 raise ValueError("prompt strings need a text_encoder/tokenizer; pass prompt_embeds instead")

@@ -1,4 +1,4 @@
-"""B200 mirror of the reference's `models/pipeline_stage2.py` `MaskedLatentToVideoPipeline.__call__` (:171-337), the
+"""Mirror of the reference's `models/pipeline_stage2.py` `MaskedLatentToVideoPipeline.__call__` (:171-337), the
 transparent-video (RGBA) generation call of `train_transparent_i2v_stage2.py:500-515` (SURVEY row f4).
 
 Relation to the main path: the denoising loop (:252-296) is `LatentToVideoPipeline.__call__`'s loop (models/pipeline.py:
@@ -46,7 +46,7 @@ class MaskedLatentToVideoPipeline(LatentToVideoPipeline):
         if vae_alpha_decoder is None:
             raise TypeError("'NoneType' object is not callable")       # what :308 raises without a decoder
         if not hasattr(vae_alpha_decoder, "decode_rgba_u8"):
-            raise TypeError("vae_alpha_decoder must be animate_anything_b200.layerdiffuse_VAE.UNet384 (the sm_100a mirror of "
+            raise TypeError("vae_alpha_decoder must be animate_anything_b200.layerdiffuse_VAE.UNet384 (the sm_90a mirror of "
                             "models/layerdiffuse_VAE.py:UNet384); a torch module would mean an eager fallback, which this "
                             "path does not have")
         _, latents = LatentToVideoPipeline.__call__(

@@ -1,7 +1,7 @@
-"""B200 mirror of the reference's `MaskStableVideoDiffusionPipeline.__call__` (models/pipeline.py:223-466; BASELINE config
+"""Mirror of the reference's `MaskStableVideoDiffusionPipeline.__call__` (models/pipeline.py:223-466; BASELINE config
 4, driven by train_svd.py:756-777): same keyword arguments, defaults and return values.
 
-What is mirrored on the sm_100a kernels (the hot path, reference line -> here):
+What is mirrored on the sm_90a kernels (the hot path, reference line -> here):
   :359-362  `_encode_vae_image` (VAE encode of the noise-augmented image, `latent_dist.mode()`)  -> AutoencoderKLTemporalDecoder.encode
   :418-422  `cat([latents] * 2)`, `scale_model_input`, `cat([mask, x, image_latents], dim=2)`       -> ONE kernel, `aab_svd_in_assemble`
   :425-431  UNetSpatioTemporalConditionModel.forward                                              -> unet_spatio_temporal_condition.py
@@ -115,7 +115,7 @@ class MaskStableVideoDiffusionPipeline:
             if cfg and image_embeddings.shape[0] == batch_size:
                 image_embeddings = torch.cat([torch.zeros_like(image_embeddings), image_embeddings])
         fps = fps - 1
-        # 4. VAE-encode the noise-augmented image (:352-362); needs_upcasting (:355) is moot: the sm_100a path is 16-bit
+        # 4. VAE-encode the noise-augmented image (:352-362); needs_upcasting (:355) is moot: the sm_90a path is 16-bit
         noise = torch.randn(image_t.shape, generator=generator, device=generator.device if generator is not None else device,
                             dtype=image_t.dtype).to(device)
         image_t = image_t + noise_aug_strength * noise
@@ -167,7 +167,7 @@ class MaskStableVideoDiffusionPipeline:
 
 
 class TextStableVideoDiffusionPipeline(MaskStableVideoDiffusionPipeline):
-    """B200 mirror of the reference's `TextStableVideoDiffusionPipeline.__call__` (models/pipeline.py:468-731): the SVD loop
+    """Mirror of the reference's `TextStableVideoDiffusionPipeline.__call__` (models/pipeline.py:468-731): the SVD loop
     conditioned on the CLIP image embedding (`condition_type="image"`), on text embeddings (`"text"`: prompt_embeds [B, 77, D]
     replace the image embedding, :579-582) or on both (any other value: image token + text tokens concatenated, 78 keys, :583-587);
     per-frame mask `[B, F, 1, h, w]` duplicated for the two CFG halves (:590), conditioning latents either from the image
@@ -199,7 +199,7 @@ class TextStableVideoDiffusionPipeline(MaskStableVideoDiffusionPipeline):
         image_t = self.image_processor.preprocess(image, height=height, width=width).to(device)
         batch_size = image_t.shape[0]
         if batch_size * num_videos_per_prompt != 1:
-            raise NotImplementedError("one video per call on the sm_100a path")
+            raise NotImplementedError("one video per call on the sm_90a path")
 
         def _text():
             if prompt_embeds is None or (cfg and negative_prompt_embeds is None):

@@ -91,7 +91,7 @@ class _Base:
         return sa * original_samples + sb * noise
 
     def step(self, model_output, timestep, sample, **kw):
-        raise NotImplementedError("the B200 pipeline fuses CFG + scheduler step into one kernel "
+        raise NotImplementedError("this pipeline fuses CFG + scheduler step into one kernel "
                                   "(LatentToVideoPipeline / ops.cfg_scheduler_step with step_coefficients()); "
                                   "a stand-alone torch step() is deliberately not provided")
 

@@ -1,5 +1,5 @@
-"""B200 mirror of the reference's `models/unet_3d_blocks.py` block classes: same class names, constructor arguments,
-sub-module attribute names (-> identical state_dict keys) and layer order, executed on the sm_100a engine.
+"""Mirror of the reference's `models/unet_3d_blocks.py` block classes: same class names, constructor arguments,
+sub-module attribute names (-> identical state_dict keys) and layer order, executed on the sm_90a engine.
 
 Layer order per the reference:
   CrossAttnDownBlock3D / CrossAttnUpBlock3D: resnet -> temp_conv -> attn -> temp_attn   (unet_3d_blocks.py:514-526,747-759)
@@ -36,7 +36,7 @@ class _Block(nn.Module):
     gradient_checkpointing = False
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("blocks are executed through UNet3DConditionModel.forward (B200 engine)")
+        raise RuntimeError("blocks are executed through UNet3DConditionModel.forward (sm_90a engine)")
 
 
 class UNetMidBlock3DCrossAttn(_Block):

@@ -1,6 +1,6 @@
-"""B200 mirror of the reference's `models/unet_3d_condition_mask.py` `UNet3DConditionModel`:
+"""Mirror of the reference's `models/unet_3d_condition_mask.py` `UNet3DConditionModel`:
 same constructor config (:87-110), same sub-module names / state_dict keys (:137-266), same `forward` signature and
-semantics (:338-526), executed as a sequence of hand-written sm_100a kernels.
+semantics (:338-526), executed as a sequence of hand-written sm_90a kernels.
 
 Forward (reference line -> here):
   :376      cat(condition_latent, sample) on the frame axis, T = F + 1      -> fused into `unet_in_assemble`
@@ -147,7 +147,7 @@ class UNet3DConditionModel(ModelBase):
         pass
 
     def enable_gradient_checkpointing(self):
-        raise NotImplementedError("training (backward) is outside the B200 inference hot path (SURVEY.md 8, component 8)")
+        raise NotImplementedError("training (backward) is outside the inference hot path (SURVEY.md 8, component 8)")
 
     # ------------------------------------------------------------------ weight preparation
     def _prepared(self) -> E.Prepared:
@@ -156,7 +156,7 @@ class UNet3DConditionModel(ModelBase):
         if prep is not None and prep.dtype == p0.dtype and prep.device == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16):
-            raise TypeError(f"the sm_100a path computes in fp16 or bf16; model dtype is {p0.dtype}. "
+            raise TypeError(f"the sm_90a path computes in fp16 or bf16; model dtype is {p0.dtype}. "
                             f"Call .to(torch.float16) / .to(torch.bfloat16). There is no fp32/CPU fallback.")
         if not p0.is_cuda:
             raise RuntimeError("UNet3DConditionModel parameters must live on a CUDA device (no CPU fallback)")

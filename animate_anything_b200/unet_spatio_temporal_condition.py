@@ -1,10 +1,10 @@
-"""B200 mirror of diffusers' `UNetSpatioTemporalConditionModel` (Stable Video Diffusion) as the reference drives it:
+"""Mirror of diffusers' `UNetSpatioTemporalConditionModel` (Stable Video Diffusion) as the reference drives it:
 `MaskStableVideoDiffusionPipeline.__call__` (models/pipeline.py:223-466; loop :416-450) feeds it the 9-channel
 `cat([mask, latents, image_latents], dim=2)` (:422) from train_svd.py:756-777 (BASELINE config 4).
 
 Same constructor config, sub-module names (-> state_dict keys) and forward signature as diffusers 0.24
 (`forward(sample [B, F, C, H, W], timestep, encoder_hidden_states [B, 1, D], added_time_ids [B, 3])` -> `.sample`
-[B, F, 4, H, W]); executed on the same sm_100a kernels as the UNet3D path:
+[B, F, 4, H, W]); executed on the same sm_90a kernels as the UNet3D path:
 
   SpatioTemporalResBlock      = ResnetBlock2D (implicit-GEMM convs, per-sample time-embedding bias in the epilogue)
                                 + TemporalResnetBlock (GroupNorm over [b, c, f, h, w] + SiLU -> 3-tap temporal implicit GEMM,
@@ -105,7 +105,7 @@ class TransformerSpatioTemporalModel(_ParamsOnly):
                  cross_attention_dim=None):
         super().__init__()
         if attention_head_dim != 64:
-            raise ValueError("the sm_100a attention kernels are specialised for head_dim 64 (SVD: 320/5, 640/10, 1280/20)")
+            raise ValueError("the sm_90a attention kernels are specialised for head_dim 64 (SVD: 320/5, 640/10, 1280/20)")
         inner = num_attention_heads * attention_head_dim
         if inner != in_channels:
             raise NotImplementedError("inner_dim != in_channels is not used by SVD")
@@ -234,7 +234,7 @@ def st_transformer_forward(ctx: E.Ctx, m: TransformerSpatioTemporalModel, x, g: 
 # ------------------------------------------------------------------------------------------------ blocks
 class _Blk(nn.Module):
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("blocks are executed through UNetSpatioTemporalConditionModel.forward (B200 engine)")
+        raise RuntimeError("blocks are executed through UNetSpatioTemporalConditionModel.forward (sm_90a engine)")
 
 
 class DownBlockSpatioTemporal(_Blk):
@@ -480,7 +480,7 @@ class UNetSpatioTemporalConditionModel(ModelBase):
         if prep is not None and prep.dtype == p0.dtype and prep.device == p0.device:
             return prep
         if p0.dtype not in (torch.float16, torch.bfloat16) or not p0.is_cuda:
-            raise TypeError("UNetSpatioTemporalConditionModel must be fp16/bf16 on a CUDA device for the sm_100a path "
+            raise TypeError("UNetSpatioTemporalConditionModel must be fp16/bf16 on a CUDA device for the sm_90a path "
                             "(train_svd.py:87 loads it in fp16 on cuda); there is no fp32/CPU fallback")
         prep = self._build_prepared(p0.dtype, p0.device)
         self.__dict__["_aab_prepared"] = prep

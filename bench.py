@@ -2,7 +2,7 @@
 """Benchmark of the hot path named by BASELINE.json: `LatentToVideoPipeline.__call__` for one 16-frame 512x512 clip,
 50 DDIM steps, CFG 9, random-init full-size UNet3D (1.41 B params) + SD VAE, bf16, synthetic inputs (config 2).
 
-  python bench.py --gpus N --steps K --warmup W          # this repo (sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W          # this repo (sm_90a kernels)
   python bench.py --impl reference --gpus N ...          # the reference's CPU path (oracle port) on the host cores
 
 A "step" of this bench = one whole pipeline call (50 denoising steps + VAE decode) = 16 denoised frames per rank.
@@ -11,8 +11,12 @@ with both halves of a pair co-located, SURVEY.md 8e), decoded frames are all-gat
 
 JSON line: `value` = frames/s with inputs resident in HBM (CUDA events, max over ranks); `e2e` = the same through the
 public API with pinned HOST inputs copied H2D every step and the decoded video read back D2H; `roofline` = achieved
-tensor TFLOP/s of the dominant kernel (tcgen05 implicit GEMM, all launches of one UNet forward timed with CUDA events)
-against the measured bf16 peak; `cpu_baseline` = the oracle timed on the host cores on a bounded sample.
+tensor TFLOP/s of the dominant kernel (wgmma implicit GEMM, all launches of one UNet forward timed with CUDA events)
+against the H100 SXM data-sheet bf16 peak; `cpu_baseline` = the oracle timed on the host cores on a bounded sample.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path returned in its last step as DIR/<name>.npy
+(float32; a fixed, seeded sample where the arrays exceed 64 MB in all).  Inputs and weights are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -35,12 +39,29 @@ SCHED = dict(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear", 
 
 
 def _peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            p = json.load(f)
-        return p["bf16_tflops_sustained"], p["hbm_gbs"], "measured (MEASURED_PEAKS.json, sustained)"
-    except Exception:
-        return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    """Dense bf16 tensor rate and HBM3 bandwidth of the H100 SXM data sheet (a 700 W card; a card set to a lower power limit
+    sustains less).  The `frac` fields computed from these are shares of the data-sheet peak, not of a measured one."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16 989 TFLOP/s, HBM3 3.35 TB/s)"
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as out_dir/<name>.npy in float32.  When the arrays exceed 64 MB in all, every array is reduced to
+    the same fixed, seeded sample of its flattened elements (sorted indices of a seeded generator), so two runs stay comparable
+    element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() * 4 for t in arrays.values())
+    keep = 1.0 if total <= DUMP_BUDGET_BYTES else DUMP_BUDGET_BYTES / total
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if keep < 1.0:
+            flat = a.reshape(-1)
+            idx = np.sort(np.random.default_rng(0).choice(flat.size, size=int(flat.size * keep), replace=False))
+            a = flat[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 class ClockSampler(threading.Thread):
@@ -322,15 +343,8 @@ def kernel_rooflines(pipe, devin, dev):
     tot_ms = sum(p["ev"][0].elapsed_time(p["ev"][1]) for p in prof)
     tot_fl = sum(p["flops"] for p in prof)
     achieved = tot_fl / (tot_ms * 1e-3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = json.load(open(tp)).get("igemm_dram_bytes_per_launch")
-        except Exception:
-            traffic = None
-    roof = {"bound": "tensor", "kernel": "aab::igemm_kernel (tcgen05 implicit GEMM, all launches of one UNet forward)",
-            "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic,
+    roof = {"bound": "tensor", "kernel": "aab::igemm_kernel (wgmma implicit GEMM, all launches of one UNet forward)",
+            "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
             "peak_source": peak_src, "launches": len(prof), "algorithmic_tflop_per_forward": tot_fl / 1e12,
             "igemm_ms_per_forward": tot_ms, "avg_launch_us": tot_ms * 1e3 / max(1, len(prof))}
     ops.KERNEL_PROFILE = []
@@ -428,6 +442,8 @@ def run_product(args):
         torch.cuda.synchronize()
         torch.cuda.profiler.stop()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"video": video, "latents": lat})
     t_dev = torch.tensor([e0.elapsed_time(e1) / 1e3], device=dev, dtype=torch.float64)
     launches = _lib.launch_count() - l0
     if pipe.use_cuda_graph:            # python-side calls happen once at capture; every replay re-launches them
@@ -507,7 +523,7 @@ def run_product(args):
                 "scaling": "strong" if latency else "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
                 "mode": args.mode if world > 1 else "throughput",
                 "config": {"workload": workload,
-                           "l2_policy": "working set per UNet forward (2.8 GB weights + activations) >> 126 MB L2",
+                           "l2_policy": "working set per UNet forward (2.8 GB weights + activations) >> 50 MB L2",
                            "cuda_graph": not args.no_graph, "finite_output": finite, "parallelism": par,
                            "parity_check": parity},
                 "unet_fwd_ms_per_step": unet_ms, "vae_decode_16f_ms": vae_ms, "clocks": sampler.summary(),
@@ -637,8 +653,14 @@ def run_svd(args):
     sampler = ClockSampler(0)
     sampler.start()
     l0 = _lib.launch_count()
-    t_dev = _ev_ms(lambda: clip(devin), reps=args.steps, warm=0) / 1e3
+    last = {}
+
+    def timed():
+        last["frames"] = clip(devin)
+    t_dev = _ev_ms(timed, reps=args.steps, warm=0) / 1e3
     launches = _lib.launch_count() - l0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"frames": last["frames"][0]})
 
     def e2e():
         inp = {k: v.to(dev, non_blocking=True) for k, v in host.items()}
@@ -660,7 +682,7 @@ def run_svd(args):
             "config": {"workload": "config4: MaskStableVideoDiffusionPipeline.__call__ 25x576x1024, 25 Euler steps, per-frame CFG "
                                    "1->3, random-init UNetSpatioTemporalConditionModel (9-ch) + AutoencoderKLTemporalDecoder, "
                                    "decode_chunk_size 8; image embedding synthetic (CLIP vision tower outside the hot path)",
-                       "l2_policy": "working set per UNet forward >> 126 MB L2", "cuda_graph": False},
+                       "l2_policy": "working set per UNet forward >> 50 MB L2", "cuda_graph": False},
             "unet_fwd_ms_per_step": unet_ms, "clocks": sampler.summary(),
             "e2e": {"value": nf / t_e2e, "unit": UNIT, "h2d_bytes_per_step": sum(v.numel() * v.element_size() for v in host.values()),
                     "d2h_bytes_per_step": nf * 3 * hh * ww},
@@ -672,7 +694,7 @@ def run_vae(args):
     """BASELINE config 5 (opt-in: `--workload vae`): VAE-only throughput sweep.  N frames (64 ... 1024) are split evenly over
     the ranks; every rank decodes its latent frames to uint8 (fused tail) and encodes as many 512x512 images; the decoded
     frames are all-gathered (the path's one collective).  Per N: frames/s (max over ranks) and achieved tensor TFLOP/s
-    against the measured peak (2.515 TFLOP per decoded frame, 1.117 per encoded frame: BASELINE.md section 4)."""
+    against the data-sheet peak (2.515 TFLOP per decoded frame, 1.117 per encoded frame: BASELINE.md section 4)."""
     import torch
     import torch.distributed as dist
     from animate_anything_b200.autoencoder_kl import AutoencoderKL
@@ -691,6 +713,7 @@ def run_vae(args):
     vae = vae.to(dtype).eval()
     peak_tf, _, peak_src = _peaks()
     rows = []
+    last = {}
     g = torch.Generator().manual_seed(3 + rank)
     for n_total in (64, 128, 256, 512, 1024):
         n = n_total // world
@@ -700,6 +723,7 @@ def run_vae(args):
 
         def decode():
             fr = vae.decode_frames_uint8(lat)
+            last["frames"] = fr
             if world > 1:
                 dist.all_gather_into_tensor(gather, fr.unsqueeze(0))
             return fr
@@ -723,9 +747,11 @@ def run_vae(args):
         del lat, img, gather
         torch.cuda.empty_cache()
     if rank == 0:
-        last = rows[-1]
-        line = {"metric": "vae_decode_frames_per_sec_512x512", "value": last["decode_frames_per_s"], "unit": UNIT,
-                "n_gpus": world, "steps": 1, "warmup": 1, "ms_per_step": 1024 / last["decode_frames_per_s"] * 1e3,
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"decoded_frames": last["frames"]})
+        top = rows[-1]
+        line = {"metric": "vae_decode_frames_per_sec_512x512", "value": top["decode_frames_per_s"], "unit": UNIT,
+                "n_gpus": world, "steps": 1, "warmup": 1, "ms_per_step": 1024 / top["decode_frames_per_s"] * 1e3,
                 "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
                 "config": {"workload": "config5: AutoencoderKL (SD VAE, random init) decode [N,4,64,64] -> uint8 512x512 frames and "
                                        "encode [N,3,512,512], N = 64..1024 split evenly over the GPUs, one all-gather of decoded frames",
@@ -751,6 +777,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="disable CUDA-graph replay of the denoising step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle parity check and the torch-eager leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (float32, <= 64 MB in all)")
     ap.add_argument("--mode", default="throughput", choices=["throughput", "latency"],
                     help="N>1 only. throughput (default, what the driver's scaling run uses): one clip per GPU. latency: "
                          "BASELINE config 3 -- N=2 one clip with its CFG halves on two GPUs; N=4 four prompts, pairs "

@@ -1,4 +1,4 @@
-/* aab200.h — C-ABI of libaab200.so: the sm_100a kernels of the animate-anything denoising hot path.
+/* aab200.h — C-ABI of libaab200.so: the sm_90a (Hopper) kernels of the animate-anything denoising hot path.
  *
  * The reference (alibaba/animate-anything) has no FFI of its own: its hot path is Python composing
  * `diffusers==0.24.0` leaf modules that bottom out in cuDNN / cuBLAS / SDPA calls.  Each entry point below is what a
@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-/* Implicit GEMM on tcgen05 (TMA-fed, TMEM accumulators): Linear, conv3x3 (pad 1), conv3x3 stride 2, Conv3d (3,1,1),
+/* Implicit GEMM on wgmma (TMA-fed, register accumulators): Linear, conv3x3 (pad 1), conv3x3 stride 2, Conv3d (3,1,1),
  * batched Q.K^T / P.V.  Replaces cuBLAS/cuDNN under diffusers ResnetBlock2D.conv1/conv2/conv_shortcut/time_emb_proj,
  * TemporalConvLayer.conv1..4, Downsample2D.conv, Upsample2D.conv, Attention.to_q/k/v/to_out, GEGLU.proj (fused gate),
  * FeedForward.net[2], Transformer*.proj_in/out, AutoencoderKL convs
@@ -32,7 +32,7 @@ int aab_igemm(const AabIgemmDesc* desc, void* stream);
  * epilogue), 0 when its epilogue cannot (direct-store variants, GEGLU) and the caller must run the statistics pass. */
 int aab_igemm_emits_colstats(const AabIgemmDesc* desc);
 
-/* Spatial self-attention / text cross-attention, head_dim 64, flash-style on tcgen05
+/* Spatial self-attention / text cross-attention, head_dim 64, flash-style on wgmma
  * (diffusers AttnProcessor2_0 -> F.scaled_dot_product_attention; installed by train.py:124-138, blocks built at
  * models/unet_3d_blocks.py:287-296,446-456,681-691).  q: [nb*lq, ldq] with head h at columns q_col0 + 64 h;
  * k, v: columns k_col0 / v_col0 of kv [nb_kv*lk, ldkv]; query batch b reads kv batch b / kv_batch_div.

@@ -1,4 +1,4 @@
-"""R1 baseline (BASELINE.md section 2): the SAME op sequence through stock PyTorch on the B200 — the oracle modules
+"""R1 baseline (BASELINE.md section 2): the SAME op sequence through stock PyTorch on the GPU — the oracle modules
 (reference composition + diffusers restatement) in bf16 with cuDNN / cuBLAS / SDPA — timed with CUDA events.
 This is a checker-side measurement (uses oracle/), not part of the product path."""
 import os

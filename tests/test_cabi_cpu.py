@@ -77,7 +77,7 @@ def test_pick_box_and_block_n():
     assert ops.pick_block_n(1280, 17) == 256          # widest tile even with fewer tiles than SMs (measured 1.7x)
     assert ops.pick_block_n(2560, 2) == 64            # GEMV-like: spread weight rows
     assert ops.pick_block_n(320, 1088, k_total=320) == 128
-    # round 2c (UNet384's 32 / 64-channel levels, profiles/r02c_alpha_tail_kernels_*.md): N <= 64 takes 64-column tiles
+    # UNet384's 32 / 64-channel levels: N <= 64 takes 64-column tiles
     assert ops.pick_block_n(64, 8192, k_total=576) == 64 and ops.pick_block_n(128, 8192, k_total=1152) == 256
 
 
@@ -164,10 +164,10 @@ def test_save_and_from_pretrained_roundtrip(tmp_path):
         assert k1 == k2 and torch.equal(v1, v2)
 
 
-def test_built_library_contains_blackwell_tensor_core_and_tma_sass():
-    """The shipped `libaab200.so` is sm_100a code whose SASS holds the 5th-generation tensor-core and TMA instructions the design
-    claims (B200_PROFILING.md mnemonics): UTCHMMA = tcgen05.mma (fp16 / bf16), LDTM = tcgen05.ld (TMEM -> registers), UTMALDG /
-    UTMASTG = cp.async.bulk.tensor load / store, UTCBAR = tcgen05.commit.  HMMA (mma.sync) only serves the T <= 32 temporal attention."""
+def test_built_library_contains_hopper_tensor_core_and_tma_sass():
+    """The shipped `libaab200.so` is sm_90a code whose SASS holds the Hopper tensor-core and TMA instructions the design
+    claims: HGMMA = wgmma.mma_async (fp16 / bf16, implicit GEMM and flash attention), UTMALDG = cp.async.bulk.tensor load,
+    WARPGROUP = the wgmma fence / commit / wait.  HMMA (mma.sync) only serves the T <= 32 temporal attention."""
     import shutil
     import subprocess
     from animate_anything_b200 import _lib
@@ -176,8 +176,7 @@ def test_built_library_contains_blackwell_tensor_core_and_tma_sass():
         import pytest
         pytest.skip("cuobjdump not available")
     arch = subprocess.run([tool, "-lelf", _lib.LIB_PATH], capture_output=True, text=True, timeout=120).stdout
-    assert "sm_100a" in arch, arch[:400]
+    assert "sm_90a" in arch, arch[:400]
     sass = subprocess.run([tool, "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=300).stdout
-    count = {m: sass.count(m) for m in ("UTCHMMA", "LDTM", "UTMALDG", "UTMASTG", "UTCBAR", "HMMA")}
-    assert count["UTCHMMA"] >= 100 and count["LDTM"] >= 40 and count["UTMALDG"] >= 50 and count["UTMASTG"] >= 10, count
-    assert count["UTCBAR"] >= 30, count
+    count = {m: sass.count(m) for m in ("HGMMA", "UTMALDG", "WARPGROUP", "HMMA")}
+    assert count["HGMMA"] >= 40 and count["UTMALDG"] >= 30 and count["WARPGROUP"] >= 20, count

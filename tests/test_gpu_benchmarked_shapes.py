@@ -2,7 +2,7 @@
 text [2,77,1024], bf16; full-size UNet3D and the full-size SD VAE), against fixtures produced by the VERBATIM reference
 files (`tests/golden/make_golden.py benchmarked`: fp32 math on bf16-rounded weights and inputs).
 
-Per stage (conv_in, transformer_in, every down/mid/up block) and for the final output the error of the sm_100a path
+Per stage (conv_in, transformer_in, every down/mid/up block) and for the final output the error of the sm_90a path
 against the fp32 oracle is ASSERTED against the yard-stick — the stock PyTorch bf16 execution (cuDNN/cuBLAS/SDPA) of the
 same op sequence on the same GPU — and every number goes into the table printed at the end of the test log."""
 import os
@@ -51,15 +51,18 @@ def test_unet_config2_bf16_forward_and_stages():
     inp = _inputs(sh["b"], sh["f"], sh["hw"], sh["lk"], sh["cdim"], dtype)
     mot = torch.tensor([gold["motion"]], device="cuda")
     t = gold["timestep"]
-    ref = gold["out"].cuda()
-    scale = ref.abs().mean().item()
+    # the fixture keeps every `out_stride`-th element of the flattened output (and the mean |out| of all of it)
+    stride = gold["out_stride"]
+    ref = gold["out_sampled"].cuda()
+    scale = gold["out_abs_mean"]
     st32, st16 = {}, {}
     hooks = _hook_stages(oracle, st32)
     with torch.no_grad():
         o32 = oracle(inp["sample"].float(), t, inp["ehs"].float(), inp["cond"].float(), inp["mask"].float(), motion=mot)
     for h in hooks:
         h.remove()
-    e_or = (o32 - ref).abs().max().item()
+    assert tuple(o32.shape) == gold["out_shape"]
+    e_or = (o32.reshape(-1)[::stride] - ref).abs().max().item()
     # the oracle restatement on the GPU (fp32, TF32 off) must reproduce the CPU output of the verbatim reference files
     assert e_or <= 5e-3 * scale, f"fp32 oracle on GPU vs verbatim-reference golden: {e_or:.3e} (|ref| {scale:.3e})"
     ours.__dict__["_trace"] = []
@@ -84,7 +87,7 @@ def test_unet_config2_bf16_forward_and_stages():
         # per-stage bar: bf16 chains of different kernel stacks decorrelate, so allow 2x the stock mean error per stage
         assert_vs_stock(row, mean_factor=2.0, max_factor=3.0, mean_floor=1e-3, max_floor=1e-2)
     assert seen == set(STAGES), f"stages not traced: {set(STAGES) - seen}"
-    row = record_parity(case, "output (golden)", out, ref, stock)
+    row = record_parity(case, "output (golden)", out.reshape(-1)[::stride], ref, stock.reshape(-1)[::stride])
     assert_vs_stock(row)
 
 
@@ -108,13 +111,16 @@ def test_vae_fullsize_bf16_encode_decode():
     frames = torch.randn(1, 1, 3, 512, 512, generator=g).clamp(-1, 1).to(dtype).cuda()
     lat = torch.randn(1, 4, 2, 64, 64, generator=g).to(dtype).cuda()
     ref_enc = gold["enc_latents"].cuda()
-    ref_vid = gold["video_f16"].float().cuda()
+    vstride = gold["video_stride"]
+    ref_vid = gold["video_f16_sampled"].float().cuda()          # every `video_stride`-th element of the flattened video
     with torch.no_grad():
         o_enc = oracle_encode_image(ovae, frames.float())
         o_vid = oracle_decode_latents(ovae, lat.float())
     # oracle on the GPU reproduces the verbatim-reference fixtures (video stored in fp16: 5e-4 relative rounding)
     assert (o_enc - ref_enc).abs().max().item() <= 5e-3 * ref_enc.abs().mean().item()
-    assert (o_vid - ref_vid).abs().max().item() <= 5e-3 * ref_vid.abs().mean().item() + 1e-3 * ref_vid.abs().max().item()
+    assert tuple(o_vid.shape) == gold["video_shape"]
+    o_vs = o_vid.reshape(-1)[::vstride]
+    assert (o_vs - ref_vid).abs().max().item() <= 5e-3 * ref_vid.abs().mean().item() + 1e-3 * gold["video_abs_max"]
     assert abs(o_vid.abs().mean().item() - gold["video_abs_mean"]) <= 1e-3 * gold["video_abs_mean"]
     enc = tensor_to_vae_latent(frames, vae)
     vid = vae.decode_video(lat)

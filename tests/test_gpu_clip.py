@@ -1,4 +1,4 @@
-"""GPU parity of the CLIP text tower (clip_text.CLIPTextModel on the sm_100a kernels) against the REAL third-party
+"""GPU parity of the CLIP text tower (clip_text.CLIPTextModel on the sm_90a kernels) against the REAL third-party
 implementation the reference imports (`transformers.CLIPTextModel`, train.py:88; installed in the image) — this leg of the
 path is pinned to the library itself, not to a restatement.  Reference call site: models/pipeline.py:136."""
 import os
@@ -69,7 +69,7 @@ def test_clip_text_matches_transformers(dtype, act, layers, hidden, heads):
 
 def test_pipeline_prompt_strings_run_on_the_kernels(monkeypatch):
     """`pipe(prompt="...")` with a transformers CLIPTextModel handed in (as train.py:799 does): the pipeline mirrors it
-    onto the sm_100a kernels; the library module's forward must never run."""
+    onto the sm_90a kernels; the library module's forward must never run."""
     from animate_anything_b200.pipeline import LatentToVideoPipeline
 
     class Tok:

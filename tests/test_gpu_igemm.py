@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM kernel against plain PyTorch fp32 on the same 16-bit-rounded inputs.
+"""GPU parity of the wgmma implicit-GEMM kernel against plain PyTorch fp32 on the same 16-bit-rounded inputs.
 Tolerance: the output is rounded once to fp16 (rel 2^-11) / bf16 (rel 2^-8) after fp32 accumulation."""
 import pytest
 import torch
@@ -176,11 +176,11 @@ def test_batched_gemm_qk():
     check("batched QK^T", out, ref, 1e-3, 1e-3)
 
 
-# ------------------------------------------------------------------------------------------------ CTA pairs (cta_group::2)
+# ------------------------------------------------------------------------------------------------ clusters sharing the weight tile
 @pytest.fixture(params=["pair", "quad"])
 def pair_mode(request):
-    """pair: clusters of 2; quad: clusters of 4 (two pairs, weight tile fetched once per cluster through TMA multicast; launches
-    with fewer than 4 m-tiles fall back to clusters of 2 by themselves)."""
+    """pair: clusters of 2; quad: clusters of 4 (each CTA fetches a slice of the weight tile and multicasts it to the others;
+    launches with fewer than 4 m-tiles fall back to clusters of 2 by themselves)."""
     ops = _ops()
     old, oldq = ops.IGEMM_PAIR, ops.IGEMM_QUAD
     ops.IGEMM_PAIR = "all"
@@ -193,9 +193,9 @@ def pair_mode(request):
 @pytest.mark.parametrize("m,k,n", [(256, 64, 256), (4096, 512, 512), (1000, 640, 1280), (139264 // 8, 320, 320),
                                    (384, 1280, 2560), (130, 320, 256), (8704, 1280, 1280), (640, 320, 576), (896, 2880, 320)])
 def test_pair_linear(pair_mode, dtype, m, k, n):
-    """256-column tiles on CTA pairs: even / odd numbers of m-tiles (130 rows = 2 tiles, 1000 = 8, 384 = 3: rank 1 of the last
-    pair stores nothing), ragged last n-tile (320 = 256 + 64), partial last m-tile; bit-identical to the single-CTA kernel
-    (same K order, same epilogue)."""
+    """256-column tiles on clusters: even / odd numbers of m-tiles (130 rows = 2 tiles, 1000 = 8, 384 = 3: the last
+    cluster's CTAs past the end store nothing), ragged last n-tile (320 = 256 + 64), partial last m-tile; bit-identical to the
+    single-CTA kernel (same K order, same epilogue)."""
     ops = pair_mode
     x = _rand((m, k), dtype, 1.0, 1)
     w = _rand((n, k), dtype, k ** -0.5, 2)
@@ -216,7 +216,7 @@ def test_pair_linear(pair_mode, dtype, m, k, n):
 def test_pair_epilogues_conv_and_geglu(pair_mode):
     ops = pair_mode
     dtype = torch.bfloat16
-    # GEGLU (values | gates split across the two CTAs of the pair)
+    # GEGLU (values | gates slices fetched by different CTAs of the cluster)
     m, k, n = 1500, 320, 2560
     x = _rand((m, k), dtype, 1.0, 1)
     w = _rand((n, k), dtype, k ** -0.5, 2)

@@ -1,4 +1,4 @@
-"""GPU parity of the SVD leg (BASELINE config 4; SURVEY rows a23 / f3): UNetSpatioTemporalConditionModel on the sm_100a
+"""GPU parity of the SVD leg (BASELINE config 4; SURVEY rows a23 / f3): UNetSpatioTemporalConditionModel on the sm_90a
 kernels against the oracle restatement (oracle/shim/diffusers/_svd.py: leaf semantics recalled from diffusers 0.24,
 PARITY UNPINNED at that level; the composition is pinned to the verbatim reference pipeline by
 tests/test_oracle_golden.py::test_svd_loop_matches_reference_pipeline).  Input layout as the reference builds it at

@@ -125,7 +125,7 @@ def test_reference_main_eval_runs_unchanged(tmp_path, monkeypatch):
         calls.append({kk: (tuple(v.shape) if torch.is_tensor(v) else v) for kk, v in k.items()})
         return orig_call(self, *a, **k)
     monkeypatch.setattr(LatentToVideoPipeline, "__call__", spy)
-    # the library CLIP forward must not run: the pipeline mirrors the encoder onto the sm_100a kernels
+    # the library CLIP forward must not run: the pipeline mirrors the encoder onto the sm_90a kernels
     monkeypatch.setattr(CLIPTextModel, "forward", lambda *a, **k: (_ for _ in ()).throw(AssertionError("library CLIP ran")))
 
     ns = dict(os=os, math=math, copy=copy, torch=torch, F=F, T=T, np=np, Image=Image, rearrange=rearrange, imageio=imageio,
@@ -167,4 +167,4 @@ def test_reference_main_eval_runs_unchanged(tmp_path, monkeypatch):
     assert written[0][1] == 4 and written[0][2] == (hh, ww, 3) and written[0][3] == np.uint8
     assert scores[0] == (1, 4, 4, hh // 8, ww // 8)
     assert os.path.exists(os.path.join("output", "demo", "prompt", "0_mask.jpg"))
-    assert _lib.launch_count() - n0 > 1000, "the sm_100a kernels did not run"
+    assert _lib.launch_count() - n0 > 1000, "the sm_90a kernels did not run"

@@ -1,5 +1,5 @@
 """GPU parity of the transparent-video branch (SURVEY row f4): `UNet384`, `LatentTransparencyOffsetEncoder`
-(models/layerdiffuse_VAE.py) and `MaskedLatentToVideoPipeline.__call__` (models/pipeline_stage2.py:171-337) on the sm_100a
+(models/layerdiffuse_VAE.py) and `MaskedLatentToVideoPipeline.__call__` (models/pipeline_stage2.py:171-337) on the sm_90a
 kernels, against (a) the outputs of the VERBATIM reference classes (tests/golden/transparent_ref.pt, fp32 math on bf16-rounded
 weights), (b) the oracle restatement in fp32 on the same GPU and (c) the stock 16-bit torch execution of the same op sequence
 as the yard-stick; plus the pieces that are new for this branch: the three boundary kernels (bit-exact), GroupNorm with 4
@@ -113,7 +113,7 @@ def _load_pair(oracle_cls, ours_cls, seed, dtype):
 
 
 def test_unet384_against_verbatim_reference_fixture():
-    """bf16 sm_100a UNet384 vs the VERBATIM models/layerdiffuse_VAE.py:UNet384 output (fp32 math, same bf16-rounded weights and
+    """bf16 sm_90a UNet384 vs the VERBATIM models/layerdiffuse_VAE.py:UNet384 output (fp32 math, same bf16-rounded weights and
     inputs), with the stock bf16 torch execution of the oracle as the yard-stick."""
     from oracle.composition import OracleUNet384
     from animate_anything_b200 import _lib

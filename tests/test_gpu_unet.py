@@ -1,4 +1,4 @@
-"""GPU parity of the B200 UNet3DConditionModel.forward against the oracle (fp32, same 16-bit-rounded weights/inputs).
+"""GPU parity of the sm_90a UNet3DConditionModel.forward against the oracle (fp32, same 16-bit-rounded weights/inputs).
 
 Three error levels are reported separately (SURVEY.md section 7 'fp16 tolerance'): per kernel (test_gpu_igemm/attention/
 norm_elem: rtol=1e-3 fp16), single forward (here), full loop (test_gpu_pipeline).  For a whole forward the yard-stick is

@@ -47,7 +47,7 @@ def north_star_violations(got, ref, rtol=1e-3, atol=1e-4):
 
 
 def record_parity(case, stage, got, ref, stock=None):
-    """One row: errors of the sm_100a path and of the stock 16-bit torch execution against the same fp32 reference."""
+    """One row: errors of the sm_90a path and of the stock 16-bit torch execution against the same fp32 reference."""
     scale = ref.float().abs().mean().item()
     mx, mean = err_stats(got, ref)
     row = {"case": case, "stage": stage, "ref_abs_mean": scale, "ours_max": mx, "ours_mean": mean,

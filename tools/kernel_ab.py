@@ -1,7 +1,7 @@
 """A/B timing of the HBM-bound kernels at the shapes of a config-2 UNet forward (one CUDA graph of 24 calls over rotating input buffers, replay timed with events: GPU-bound like
 the pipeline's graph replay; a call never finds its own input of the previous iteration in L2).  Variants are selected per PROCESS by the env
 switches read in csrc (AAB_GN_TWO_PASS=1, AAB_LN_V1=1, AAB_TATTN_V1=1); run it twice to compare.
-    python tools/kernel_ab.py [gn|ln|ta|fa|all]      (fa: text cross-attention; AAB_FLASH_NO_SHORT=1 = round-1 kernel)
+    python tools/kernel_ab.py [gn|ln|ta|fa|all]      (fa: text cross-attention)
 """
 import os
 import sys
@@ -45,7 +45,7 @@ def timeit(fn, nbuf, iters=24):
     return e0.elapsed_time(e1) / (3 * iters) * 1e3      # us
 
 
-tag = ",".join(k for k in ("AAB_LN_V1", "AAB_TATTN_V1", "AAB_FLASH_NO_SHORT") if os.environ.get(k) == "1") or "round-2 kernels"
+tag = ",".join(k for k in ("AAB_LN_V1", "AAB_TATTN_V1") if os.environ.get(k) == "1") or "round-2 kernels"
 print(f"variant: {tag}")
 print("| kernel | shape | us / call | algorithmic GB/s | frac of 6485.5 |")
 print("|---|---|---|---|---|")

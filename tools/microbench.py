@@ -89,8 +89,7 @@ if "ln" in names:
     timeit("layernorm [139264,320]", lambda: ops.layernorm(x, ga, be), bytes_=2 * M * 320 * 2)
 
 if "gn_shapes" in names:
-    # every GroupNorm extent of config 2 (2-D per frame, 3-D per clip, concat widths, VAE decoder).  The sweep in
-    # profiles/r01_gn_chunk_sweep.md was taken with a temporary override of the elements-per-CTA target in norm.cu.
+    # every GroupNorm extent of config 2 (2-D per frame, 3-D per clip, concat widths, VAE decoder)
     shapes = [(32, 4096, 320), (32, 1024, 640), (32, 256, 1280), (32, 64, 1280), (32, 4096, 640), (32, 1024, 1280),
               (2, 65536, 320), (2, 16384, 640), (2, 4096, 1280), (2, 1024, 1280), (1, 65536, 320), (1, 16384, 640), (8, 262144, 128)]
     for (s_, r_, c_) in shapes:
