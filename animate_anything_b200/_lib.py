@@ -49,6 +49,13 @@ _SIGS = {
                            C.c_void_p, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int,
                            C.c_void_p, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                            C.c_float, C.c_int, C.c_void_p],
+    "aab_flash_attn_d80": [C.c_void_p, C.c_long, C.c_long, C.c_int, C.c_int,
+                           C.c_void_p, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int,
+                           C.c_void_p, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                           C.c_float, C.c_int, C.c_void_p],
+    "aab_clip_image_prep": [C.c_void_p, C.c_int, C.c_long, C.c_long, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int,
+                            C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_long,
+                            C.c_int, C.c_void_p],
     "aab_temporal_attn_d64": [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_long, C.c_int, C.c_int,
                               C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p],
     "aab_groupnorm": [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_long, C.c_int, C.c_long, C.c_long, C.c_int,

@@ -9,6 +9,9 @@
 //    O += P.V (wgmma, V MN-major in shared memory).  64-key K/V blocks are TMA-loaded into a 3-stage ring by a producer
 //    warp.  Keys past Lk (e.g. 77 text tokens) are masked to -inf.
 //
+// 1b. aab_flash_attn_d80 — the same kernel for head_dim 80, bidirectional: the self-attention of the CLIP ViT-H/14 image
+//    tower (transformers CLIPAttention, 257 tokens) behind the SVD pipelines' `_encode_image` (models/pipeline.py:347,597).
+//
 // 2. aab_temporal_attn_d64 — self-attention over the frame axis (T <= 32) of TransformerTemporalModel
 //    (models/unet_3d_blocks.py:299-306,459-467,694-701; called without encoder_hidden_states so both attn1 and attn2
 //    are self-attention over T).  Activations stay in [B, T, H*W, C] order; the kernel gathers the T rows of one
@@ -189,6 +192,180 @@ flash_attn_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                      2 * (lane & 3)) * 2;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(op + jj * 16) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, BF16);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ head dim 80
+// The CLIP ViT-H/14 image tower (transformers CLIPVisionModelWithProjection: 16 heads of 80, 257 tokens, bidirectional).
+// Same pipeline as flash_attn_d64_kernel; what differs is the shared-memory layout.  A row of 80 16-bit values is 160 B and
+// does not fit one 128-byte swizzle atom, so every operand is TMA-loaded as five 16-column boxes with SWIZZLE_32B (32-byte
+// rows): S = Q.K^T is five k16 steps, one per box pair, and O += P.V runs per 16-column chunk of V (m64n16k16), so the
+// O accumulator is five 8-register chunks (40 fp32 registers per thread).
+constexpr int FA80_CHUNKS = 5;                               // 16-column boxes per head
+constexpr int FA80_Q_CHUNK = 128 * 32;                       // [128 rows x 16] 16-bit
+constexpr int FA80_KV_CHUNK = FA_BKV * 32;                   // [64 rows x 16] 16-bit
+constexpr int FA80_Q_BYTES = FA80_CHUNKS * FA80_Q_CHUNK;     // 20 KiB
+constexpr int FA80_KV_BYTES = FA80_CHUNKS * FA80_KV_CHUNK;   // 10 KiB
+constexpr int FA80_SMEM_BYTES = FA80_Q_BYTES + FA_KV_STAGES * 2 * FA80_KV_BYTES + 1024 + 256;
+
+template <bool BF16>
+__global__ void __launch_bounds__(FA_THREADS, 2)
+flash_attn_d80_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const FaParams p) {
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smQ = smem;                                    // [5][128 x 16]
+  uint8_t* smK = smQ + FA80_Q_BYTES;                      // [ST][5][64 x 16]
+  uint8_t* smV = smK + FA_KV_STAGES * FA80_KV_BYTES;      // [ST][5][64 x 16]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smV + FA_KV_STAGES * FA80_KV_BYTES);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;
+  uint64_t* kv_empty = kv_full + FA_KV_STAGES;
+
+  const int warp = static_cast<int>(threadIdx.x) >> 5;
+  const int q0 = blockIdx.x * 128;
+  const int head = blockIdx.y;
+  const int b = blockIdx.z;
+  const int bkv = b / p.kv_batch_div;
+  const int nkv = (p.Lk + FA_BKV - 1) / FA_BKV;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmQ);
+    prefetch_tmap(&tmKV);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < FA_KV_STAGES; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 8);         // lane 0 of each consumer warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == 8) {
+    if (elect_one()) {
+      mbar_arrive_expect_tx(q_full, FA80_Q_BYTES);
+      for (int c = 0; c < FA80_CHUNKS; ++c)
+        tma_load_3d(smQ + c * FA80_Q_CHUNK, &tmQ, q_full, p.q_col0 + head * 80 + 16 * c, q0, b);
+      for (int j = 0; j < nkv; ++j) {
+        const int s = j % FA_KV_STAGES;
+        mbar_wait(&kv_empty[s], ((j / FA_KV_STAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * FA80_KV_BYTES);
+        for (int c = 0; c < FA80_CHUNKS; ++c) {
+          tma_load_3d(smK + s * FA80_KV_BYTES + c * FA80_KV_CHUNK, &tmKV, &kv_full[s], p.k_col0 + head * 80 + 16 * c,
+                      j * FA_BKV, bkv);
+          tma_load_3d(smV + s * FA80_KV_BYTES + c * FA80_KV_CHUNK, &tmKV, &kv_full[s], p.v_col0 + head * 80 + 16 * c,
+                      j * FA_BKV, bkv);
+        }
+      }
+    }
+    return;
+  }
+
+  const int cw = warp >> 2;                   // consumer warpgroup: query rows q0 + 64 cw ...
+  const int wq = warp & 3;
+  const int lane = static_cast<int>(lane_id());
+  const int row0 = 64 * cw + 16 * wq + (lane >> 2);     // tile rows row0 and row0 + 8
+  float o[40];                                // chunk c (head columns 16c ...) in o[8c .. 8c + 8)
+#pragma unroll
+  for (int i = 0; i < 40; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t qa = smem_u32(smQ + cw * 64 * 32);
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < nkv; ++j) {
+    const int s = j % FA_KV_STAGES;
+    mbar_wait(&kv_full[s], (j / FA_KV_STAGES) & 1);
+    const uint32_t ka = smem_u32(smK + s * FA80_KV_BYTES);
+    const uint32_t va = smem_u32(smV + s * FA80_KV_BYTES);
+    // The 64-key block is consumed as two 32-key halves (S is 16 registers, not 32): with the 40-register O accumulator a
+    // full 64-key S does not fit the register budget of two 288-thread CTAs per SM without spilling.
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      // ---------------- S = Q K^T   [64 x 32 keys], one k16 step per 16-column box
+      float sc[16];
+      uint32_t qa_i = qa;
+      asm volatile("" : "+r"(qa_i));        // keeps the five loop-invariant Q descriptors from being hoisted into 10 registers
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < FA80_CHUNKS; ++c)
+        wgmma_ss<32, BF16>(sc, make_desc_sw32(qa_i + c * FA80_Q_CHUNK), make_desc_sw32(ka + c * FA80_KV_CHUNK + hf * 32 * 32),
+                           c > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs<16>(sc);
+      // ---------------- mask keys past Lk
+      const int kbase = j * FA_BKV + 32 * hf;
+      if (p.Lk - kbase < 32) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int key = kbase + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          if (key >= p.Lk) sc[i] = -INFINITY;
+        }
+      }
+      // ---------------- online softmax on the two rows of this thread (a row's 32 keys live in the 4 lanes of a quad)
+      float alpha[2], m_new[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+          if (((i >> 1) & 1) == h) mx = fmaxf(mx, sc[i]);
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        // a fully masked half (Lk <= 32 in the last block) keeps the running max, which key 0 has already made finite
+        m_new[h] = fmaxf(m_run[h], mx * p.scale_log2);
+        alpha[h] = fast_exp2(m_run[h] - m_new[h]);
+        m_run[h] = m_new[h];
+      }
+      float lsum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int h = (i >> 1) & 1;
+        sc[i] = fast_exp2(fmaf(sc[i], p.scale_log2, -m_new[h]));
+        lsum[h] += sc[i];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + lsum[h];
+#pragma unroll
+      for (int i = 0; i < 40; ++i) o[i] *= alpha[(i >> 1) & 1];
+      // ---------------- O += P V: P (16-bit) as the register A operand, 16 keys x 16 head columns per wgmma
+      uint32_t pf[2][4];
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        pf[kk][0] = pack2(sc[8 * kk + 0], sc[8 * kk + 1], BF16);
+        pf[kk][1] = pack2(sc[8 * kk + 2], sc[8 * kk + 3], BF16);
+        pf[kk][2] = pack2(sc[8 * kk + 4], sc[8 * kk + 5], BF16);
+        pf[kk][3] = pack2(sc[8 * kk + 6], sc[8 * kk + 7], BF16);
+      }
+      fence_regs<40>(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+        for (int c = 0; c < FA80_CHUNKS; ++c)
+          wgmma_rs_tb<16, BF16>(o + 8 * c, pf[kk], make_desc_sw32(va + c * FA80_KV_CHUNK + (32 * hf + 16 * kk) * 32));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs<40>(o);
+    }
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+  // ---------------- normalise and store (o[4 jj + 2 h + e] is column 8 jj + 2 (lane & 3) + e of row row0 + 8 h)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    const int q = q0 + row0 + 8 * h;
+    if (q < p.Lq) {
+      const float inv = 1.0f / l_run[h];
+      uint8_t* op = reinterpret_cast<uint8_t*>(p.out) +
+                    (static_cast<long>(b) * p.out_batch_stride + static_cast<long>(q) * p.ld_out + p.out_col0 + head * 80 +
+                     2 * (lane & 3)) * 2;
+#pragma unroll
+      for (int jj = 0; jj < 10; ++jj)
         *reinterpret_cast<uint32_t*>(op + jj * 16) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, BF16);
     }
   }
@@ -608,6 +785,61 @@ extern "C" int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, 
     static std::atomic<unsigned long long> attr_h{0};
     if (int r = ensure_dyn_smem(flash_attn_d64_kernel<false>, FA_SMEM_BYTES, attr_h)) return r;
     launch_k(flash_attn_d64_kernel<false>, grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
+  }
+  return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
+}
+
+extern "C" int aab_flash_attn_d80(const void* q, long ldq, long q_batch_stride, int q_cols, int q_col0,
+                                  const void* kv, long ldkv, long kv_batch_stride, int kv_cols, int k_col0, int v_col0,
+                                  void* out, long ld_out, long out_batch_stride, int out_col0, int nb, int nb_kv,
+                                  int kv_batch_div, int heads, int lq, int lk, float scale, int is_bf16, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (is_bf16 != 0 && is_bf16 != 1) return AAB_ERR_ARG;           // no causal variant: the vision tower is bidirectional
+  if (!q || !kv || !out || lq < 1 || lk < 1 || heads < 1 || nb < 1 || nb_kv < 1 || kv_batch_div < 1) return AAB_ERR_ARG;
+  if ((ldq % 8) || (ldkv % 8) || (ld_out % 8) || (out_col0 % 8) || (q_batch_stride % 8) || (kv_batch_stride % 8) ||
+      (reinterpret_cast<uintptr_t>(q) % 16) || (reinterpret_cast<uintptr_t>(kv) % 16) || (reinterpret_cast<uintptr_t>(out) % 16))
+    return AAB_ERR_ARG;                                            // TMA: 16-byte aligned bases and row strides
+  if (q_col0 < 0 || k_col0 < 0 || v_col0 < 0 || q_col0 + 80 * heads > q_cols || k_col0 + 80 * heads > kv_cols ||
+      v_col0 + 80 * heads > kv_cols || (nb - 1) / kv_batch_div >= nb_kv)
+    return AAB_ERR_ARG;
+  CUtensorMap tmQ, tmKV;
+  {
+    long dims[3] = {q_cols, lq, nb};
+    long strides[3] = {1, ldq, q_batch_stride};
+    int box[3] = {16, 128, 1};
+    int r = make_tmap_16(&tmQ, q, 3, dims, strides, box, is_bf16, 32);
+    if (r) return r;
+  }
+  {
+    long dims[3] = {kv_cols, lk, nb_kv};
+    long strides[3] = {1, ldkv, kv_batch_stride};
+    int box[3] = {16, FA_BKV, 1};
+    int r = make_tmap_16(&tmKV, kv, 3, dims, strides, box, is_bf16, 32);
+    if (r) return r;
+  }
+  FaParams p;
+  p.Lq = lq;
+  p.Lk = lk;
+  p.heads = heads;
+  p.kv_batch_div = kv_batch_div;
+  p.q_col0 = q_col0;
+  p.k_col0 = k_col0;
+  p.v_col0 = v_col0;
+  p.out = out;
+  p.ld_out = ld_out;
+  p.out_batch_stride = out_batch_stride;
+  p.out_col0 = out_col0;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.causal = 0;
+  const dim3 grid((lq + 127) / 128, heads, nb);
+  if (is_bf16) {
+    static std::atomic<unsigned long long> attr_b{0};
+    if (int r = ensure_dyn_smem(flash_attn_d80_kernel<true>, FA80_SMEM_BYTES, attr_b)) return r;
+    launch_k(flash_attn_d80_kernel<true>, grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream, tmQ, tmKV, p);
+  } else {
+    static std::atomic<unsigned long long> attr_h{0};
+    if (int r = ensure_dyn_smem(flash_attn_d80_kernel<false>, FA80_SMEM_BYTES, attr_h)) return r;
+    launch_k(flash_attn_d80_kernel<false>, grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream, tmQ, tmKV, p);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }

@@ -207,6 +207,17 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t
 }
 __device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) { return make_desc_sw128(smem_addr, 16); }
 __device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr) { return make_desc_sw128(smem_addr, 1024); }
+// Same for a tile stored as rows of 32 bytes (16 x 16-bit) with TMA SWIZZLE_32B: 8-row groups are 256 B apart, layout 3.
+// One k16 step of a K-major operand is the whole row; an MN-major operand of MN extent 16 needs no second chunk, so both
+// offsets are 256 (the 8-row K groups).
+__device__ __forceinline__ uint64_t make_desc_sw32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(256 >> 4) << 16;
+  d |= static_cast<uint64_t>(256 >> 4) << 32;
+  d |= static_cast<uint64_t>(3) << 62;
+  return d;
+}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

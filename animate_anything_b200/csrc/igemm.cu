@@ -398,7 +398,9 @@ int make_tmap_16(CUtensorMap* out, const void* base, int rank, const long* dims,
   CUresult r = enc(out, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
                    static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   swizzle_bytes == 32   ? CU_TENSOR_MAP_SWIZZLE_32B
+                   : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                         : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? AAB_OK : AAB_ERR_DRIVER;

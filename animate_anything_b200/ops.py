@@ -335,6 +335,54 @@ def flash_attn_d64(q: torch.Tensor, q_col0: int, kv: torch.Tensor, k_col0: int, 
     return out
 
 
+def flash_attn_d80(q: torch.Tensor, q_col0: int, kv: torch.Tensor, k_col0: int, v_col0: int, nb: int, lq: int, lk: int,
+                   heads: int, kv_batch_div: int = 1, out: Optional[torch.Tensor] = None,
+                   scale: Optional[float] = None) -> torch.Tensor:
+    """Bidirectional attention with head dim 80 (CLIP ViT-H/14 image tower).  q: [nb*lq, q_cols]; kv: [nb_kv*lk, kv_cols];
+    head h uses columns col0 + 80*h.  Returns [nb*lq, heads*80].  `scale`: softmax scale, default 1/sqrt(80)."""
+    bf = _is_bf16(q)
+    if out is None:
+        out = torch.empty((nb * lq, heads * 80), device=q.device, dtype=q.dtype)
+    nb_kv = kv.shape[0] // lk
+    _profiled("flash_attn_d80", 2.0 * 80 * heads * (2 * nb * lq + 2 * nb_kv * lk), 4.0 * nb * heads * lq * lk * 80,
+              lambda: _lib.call("aab_flash_attn_d80", _ptr(q), q.stride(0), lq * q.stride(0), q.shape[1], q_col0,
+                                _ptr(kv), kv.stride(0), lk * kv.stride(0), kv.shape[1], k_col0, v_col0,
+                                _ptr(out), out.stride(0), lq * out.stride(0), 0, nb, nb_kv, kv_batch_div, heads, lq, lk,
+                                1.0 / math.sqrt(80.0) if scale is None else float(scale), bf, _stream()),
+              shape=(nb, heads, lq, lk))
+    return out
+
+
+_SRC_TYPES = {torch.uint8: 0, torch.float32: 1, torch.float16: 2, torch.bfloat16: 3}
+
+
+def clip_image_prep(src: torch.Tensor, dtype, out_size: int, patch: int, k_pad: int, taps_y: Optional[torch.Tensor] = None,
+                    taps_x: Optional[torch.Tensor] = None, mean_std: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """CLIP image preprocessing + patchify (`aab_clip_image_prep`).  `src`: uint8 images [B, H, W, 3] (full preprocessing:
+    blur taps and mean/std as fp32 device tensors) or CLIP pixel values [B, 3, S, S] of any float dtype (rounding only).
+    Returns the patch-embedding GEMM operand [B * (1 + (S/patch)^2), k_pad] in `dtype`: row 0 of each image is the zero
+    class slot, then the patches, columns >= 3 patch^2 zero."""
+    if src.dtype not in _SRC_TYPES:
+        raise TypeError(f"image source must be uint8 or float, got {src.dtype}")
+    if src.dtype == torch.uint8:
+        b, h, w, c = src.shape
+        sb, sy, sx, sc = src.stride()
+        assert taps_y is not None and taps_x is not None and mean_std is not None
+        for t in (taps_y, taps_x, mean_std):
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.device == src.device
+    else:
+        b, c, h, w = src.shape
+        sb, sc, sy, sx = src.stride()
+    if c != 3:
+        raise ValueError(f"CLIP images have 3 channels, got {c}")
+    grid = out_size // patch
+    out = torch.empty((b * (1 + grid * grid), k_pad), device=src.device, dtype=dtype)
+    _lib.call("aab_clip_image_prep", _ptr(src), _SRC_TYPES[src.dtype], sb, sc, sy, sx, b, h, w, _ptr(taps_y),
+              0 if taps_y is None else taps_y.numel(), _ptr(taps_x), 0 if taps_x is None else taps_x.numel(), _ptr(mean_std),
+              out_size, patch, _ptr(out), out.stride(0), 1 if dtype == torch.bfloat16 else 0, _stream())
+    return out
+
+
 def temporal_attn_d64(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
     bf = _is_bf16(qkv)
     out = torch.empty((qkv.shape[0], heads * 64), device=qkv.device, dtype=qkv.dtype)

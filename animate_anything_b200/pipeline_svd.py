@@ -7,8 +7,12 @@ What is mirrored on the sm_90a kernels (the hot path, reference line -> here):
   :425-431  UNetSpatioTemporalConditionModel.forward                                              -> unet_spatio_temporal_condition.py
   :434-439  per-frame guidance (`linspace(min, max, F)`, :405-408) + EulerDiscreteScheduler.step  -> ONE kernel, `aab_svd_cfg_euler_step`
   :456      `decode_latents` in chunks of `decode_chunk_size` frames                                -> decode_chunk_video
-What stays a library call: the CLIP *vision* tower of `_encode_image` (:343; once per clip, outside SURVEY.md 8's rows) — any
-module mapping the image batch to embeddings (`.image_embeds` or a tensor) is accepted, or pass `image_embeddings=`.
+  :347      `_encode_image` with a CLIP image tower (ours or a `transformers.CLIPVisionModelWithProjection`, mirrored once) on
+            the caller's image, as diffusers 0.24 does: PIL -> resize with antialiasing to 224 + CLIP normalisation +
+            patchify in ONE kernel (`aab_clip_image_prep`), then the ViT tower on the kernels (clip_vision.py); a tensor is
+            taken as the CLIP pixel values
+Any other `image_encoder` module (mapping the VAE-preprocessed image batch to `.image_embeds` or a tensor) is called as it is,
+or pass `image_embeddings=`.
 """
 from __future__ import annotations
 
@@ -53,10 +57,60 @@ class MaskStableVideoDiffusionPipeline:
         if height % 8 != 0 or width % 8 != 0:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
 
-    def _encode_image(self, image, device, num_videos_per_prompt, do_classifier_free_guidance):
-        """CLIP image embedding [B, 1, D]; under CFG returns cat([zeros, embeddings]) (diffusers _encode_image)."""
+    def _clip_image_encoder(self):
+        """The image encoder as an sm_90a `clip_vision.CLIPVisionModelWithProjection`, or None when it is another module.
+        A `transformers.CLIPVisionModelWithProjection` is mirrored once (same weights, dtype, device); the mirror is rebuilt
+        if the caller swaps or moves the encoder."""
+        from .clip_vision import CLIPVisionModelWithProjection
+        enc = self.image_encoder
+        if isinstance(enc, CLIPVisionModelWithProjection):
+            return enc
+        if type(enc).__name__ != "CLIPVisionModelWithProjection" or not type(enc).__module__.startswith("transformers"):
+            return None
+        p0 = next(enc.parameters())
+        key = (id(enc), p0.data_ptr(), p0.dtype, p0.device)
+        cached = self.__dict__.get("_ie_mirror")
+        if cached is None or cached[0] != key:
+            cached = (key, CLIPVisionModelWithProjection.from_hf(enc))
+            self.__dict__["_ie_mirror"] = cached
+        return cached[1]
+
+    def _clip_image_embeds(self, enc, image, device):
+        """diffusers 0.24 `_encode_image` up to `.image_embeds` on the caller's image: PIL images (or a list of them, or
+        uint8 HWC arrays) go through `pil_to_numpy` -> [-1, 1] -> `_resize_with_antialiasing` -> [0, 1] -> the
+        feature extractor's normalisation, all in `aab_clip_image_prep`; a tensor is the CLIP pixel values."""
+        import numpy as np
+        import PIL.Image
+        from .clip_vision import OPENAI_CLIP_MEAN, OPENAI_CLIP_STD
+        if isinstance(image, torch.Tensor):
+            return enc(image.to(device)).image_embeds
+        images = image if isinstance(image, list) else [image]
+        arrs = []
+        for im in images:
+            if isinstance(im, PIL.Image.Image):
+                if im.mode != "RGB":
+                    raise ValueError(f"CLIP image encoding needs RGB images, got PIL mode {im.mode!r}")
+                im = np.array(im)
+            if not (isinstance(im, np.ndarray) and im.dtype == np.uint8 and im.ndim == 3 and im.shape[-1] == 3):
+                raise NotImplementedError("CLIP image encoding takes PIL RGB images, uint8 [H, W, 3] arrays or CLIP pixel "
+                                          "value tensors")
+            arrs.append(im)
+        u8 = torch.from_numpy(np.stack(arrs)).to(device)
+        fe = self.feature_extractor
+        mean = getattr(fe, "image_mean", None) or OPENAI_CLIP_MEAN
+        std = getattr(fe, "image_std", None) or OPENAI_CLIP_STD
+        return enc.encode_images(u8, mean, std).image_embeds
+
+    def _encode_image(self, image, device, num_videos_per_prompt, do_classifier_free_guidance, raw_image=None):
+        """CLIP image embedding [B, 1, D]; under CFG returns cat([zeros, embeddings]) (diffusers _encode_image).  A CLIP
+        image tower encodes `raw_image`, the caller's image (models/pipeline.py:347 passes it before the VAE
+        preprocessing); any other module gets `image`, the VAE-preprocessed batch."""
         dtype = self.unet.dtype
-        out = self.image_encoder(image.to(device=device, dtype=next(self.image_encoder.parameters()).dtype))
+        enc = self._clip_image_encoder() if raw_image is not None else None
+        if enc is not None:
+            out = self._clip_image_embeds(enc, raw_image, device)
+        else:
+            out = self.image_encoder(image.to(device=device, dtype=next(self.image_encoder.parameters()).dtype))
         emb = out.image_embeds if hasattr(out, "image_embeds") else out
         emb = emb.to(dtype).unsqueeze(1)
         bs, seq, _ = emb.shape
@@ -103,13 +157,13 @@ class MaskStableVideoDiffusionPipeline:
         device = self.unet.device
         dtype = self.unet.dtype
         cfg = max_guidance_scale > 1.0
-        # 3. image embedding (library call, once per clip) unless supplied
+        # 3. image embedding (once per clip) unless supplied
         image_t = self.image_processor.preprocess(image, height=height, width=width).to(device)
         batch_size = image_t.shape[0]
         if batch_size * num_videos_per_prompt != 1:
             raise NotImplementedError("the reference's mask handling ('1 h w -> 2 f 1 h w', :372) implies one video per call")
         if image_embeddings is None:
-            image_embeddings = self._encode_image(image_t, device, num_videos_per_prompt, cfg)
+            image_embeddings = self._encode_image(image_t, device, num_videos_per_prompt, cfg, raw_image=image)
         else:
             image_embeddings = image_embeddings.to(device=device, dtype=dtype)
             if cfg and image_embeddings.shape[0] == batch_size:
@@ -209,7 +263,7 @@ class TextStableVideoDiffusionPipeline(MaskStableVideoDiffusionPipeline):
 
         def _img():
             if image_embeddings is None:
-                return self._encode_image(image_t, device, num_videos_per_prompt, cfg)
+                return self._encode_image(image_t, device, num_videos_per_prompt, cfg, raw_image=image)
             e = image_embeddings.to(device=device, dtype=dtype)
             return torch.cat([torch.zeros_like(e), e]) if cfg and e.shape[0] == batch_size else e
 

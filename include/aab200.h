@@ -44,6 +44,28 @@ int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, int q_cols,
                        long out_batch_stride, int out_col0, int nb, int nb_kv, int kv_batch_div, int heads, int lq, int lk,
                        float scale, int is_bf16, void* stream);
 
+/* The same attention for head_dim 80, bidirectional (no causal bit: `is_bf16` must be 0 or 1): the self-attention of the CLIP
+ * ViT-H/14 image tower (transformers CLIPAttention, 16 heads x 80, 257 tokens) that the SVD pipelines' `_encode_image` runs
+ * (models/pipeline.py:347,597).  Same arguments as aab_flash_attn_d64 with head h at columns col0 + 80 h; additionally
+ * col0 + 80 heads must fit the given column counts, q / kv / out 16-byte aligned, batch strides multiples of 8. */
+int aab_flash_attn_d80(const void* q, long ldq, long q_batch_stride, int q_cols, int q_col0, const void* kv, long ldkv,
+                       long kv_batch_stride, int kv_cols, int k_col0, int v_col0, void* out, long ld_out,
+                       long out_batch_stride, int out_col0, int nb, int nb_kv, int kv_batch_div, int heads, int lq, int lk,
+                       float scale, int is_bf16, void* stream);
+
+/* CLIP image preprocessing + patchify, the input of the CLIP image tower's patch-embedding GEMM (diffusers 0.24
+ * StableVideoDiffusionPipeline._encode_image, models/pipeline.py:347,597; restated at train_svd.py:384-395).
+ * src [b, 3, h, w] by element strides; src_type 0 = uint8 (a PIL image: strides h*w*3, 1, w*3, 3), 1 = float32, 2 = float16,
+ * 3 = bfloat16.  uint8: x = u8/255, 2x - 1, separable Gaussian blur with reflect padding (taps_x [ks_x] along x first, then
+ * taps_y [ks_y] along y; fp32, odd sizes), bicubic resize (align_corners) to out_size^2, (x + 1)/2, (x - mean)/std with
+ * mean_std = fp32 [mean r, g, b, std r, g, b] -- all in fp32.  Float sources are the CLIP pixel values themselves
+ * (h == w == out_size; taps and mean_std unused): rounding only.
+ * out [b * (1 + (out_size/patch)^2), ld_out] 16-bit: row 0 of each image's block is zeros (the class-token slot), row 1 + p
+ * is patch p (row-major grid) in the column order of patch_embedding.weight.flatten(1); columns >= 3 patch^2 are zeros. */
+int aab_clip_image_prep(const void* src, int src_type, long sb, long sc, long sy, long sx, int b, int h, int w,
+                        const float* taps_y, int ks_y, const float* taps_x, int ks_x, const float* mean_std, int out_size,
+                        int patch, void* out, long ld_out, int is_bf16, void* stream);
+
 /* Self-attention over the frame axis (T <= 32) without the (b t) c h w -> (b h w) t c permutes
  * (diffusers TransformerTemporalModel.forward; models/unet_3d_blocks.py:299-306,459-467,694-701). */
 int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k_col0, int v_col0, void* out, long ld_out, int b, int t,
