@@ -744,8 +744,14 @@ extern "C" int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, 
   const int causal = (is_bf16 >> 1) & 1;
   is_bf16 &= 1;
   if (causal && (lq != lk || lk > 128)) return AAB_ERR_ARG;
-  if (!q || !kv || !out || lq < 1 || lk < 1 || heads < 1 || nb < 1 || kv_batch_div < 1) return AAB_ERR_ARG;
-  if ((ldq % 8) || (ldkv % 8) || (ld_out % 8) || (out_col0 % 8)) return AAB_ERR_ARG;
+  if (!q || !kv || !out || lq < 1 || lk < 1 || heads < 1 || nb < 1 || nb_kv < 1 || kv_batch_div < 1) return AAB_ERR_ARG;
+  if ((ldq % 8) || (ldkv % 8) || (ld_out % 8) || (out_col0 % 8) || (q_batch_stride % 8) || (kv_batch_stride % 8) ||
+      (reinterpret_cast<uintptr_t>(q) % 16) || (reinterpret_cast<uintptr_t>(kv) % 16) || (reinterpret_cast<uintptr_t>(out) % 16))
+    return AAB_ERR_ARG;                                            // TMA: 16-byte aligned bases and row strides
+  // a head or a K/V batch outside the described tensors would be read as TMA zero fill: silently wrong attention
+  if (q_col0 < 0 || k_col0 < 0 || v_col0 < 0 || q_col0 + 64 * heads > q_cols || k_col0 + 64 * heads > kv_cols ||
+      v_col0 + 64 * heads > kv_cols || (nb - 1) / kv_batch_div >= nb_kv)
+    return AAB_ERR_ARG;
   CUtensorMap tmQ, tmK, tmV;
   {
     long dims[3] = {q_cols, lq, nb};
@@ -848,7 +854,12 @@ extern "C" int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k
                                      long ld_out, int b, int t, int hw, int heads, float scale, int is_bf16,
                                      void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!qkv || !out || t < 1 || t > 32 || (ld % 8) || (ld_out % 8)) return AAB_ERR_ARG;
+  if (!qkv || !out || t < 1 || t > 32 || b < 1 || hw < 1 || heads < 1 || (ld % 8) || (ld_out % 8)) return AAB_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(qkv) % 16) || (reinterpret_cast<uintptr_t>(out) % 16) || ((q_col0 | k_col0 | v_col0) % 8))
+    return AAB_ERR_ARG;                   // 16-byte pieces (cp.async gather, row stores)
+  if (q_col0 < 0 || k_col0 < 0 || v_col0 < 0 || q_col0 + 64L * heads > ld || k_col0 + 64L * heads > ld ||
+      v_col0 + 64L * heads > ld || 64L * heads > ld_out)
+    return AAB_ERR_ARG;                   // every head's 64 columns inside a row of qkv / out
   const long total = static_cast<long>(b) * hw * heads;
   static int use_v1 = -1;                 // AAB_TATTN_V1=1: the round-1 kernel (A/B measurements)
   if (use_v1 < 0) {
@@ -856,7 +867,6 @@ extern "C" int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k
     use_v1 = (e && e[0] == '1') ? 1 : 0;
   }
   if (!use_v1) {
-    if ((q_col0 | k_col0 | v_col0) % 8) return AAB_ERR_ARG;     // 16-byte cp.async pieces
     const size_t smem2 = static_cast<size_t>(4) * 2 * TA_WARP_HALVES * sizeof(uint16_t);   // 108 KiB: double-buffered Q, K, V
     static std::atomic<unsigned long long> a2t{0}, a2f{0};
     if (int r = ensure_dyn_smem(temporal_attn_d64_v2_kernel<true>, static_cast<int>(smem2), a2t)) return r;

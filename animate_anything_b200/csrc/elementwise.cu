@@ -395,8 +395,10 @@ __global__ void add_rowvec_kernel(const void* x, long ldx, void* out, long ldo, 
   *px = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-// out = a * x + b * y with torch's 16-bit roundings of each product and of the sum (diffusers AlphaBlender.forward:
-// `alpha * x_spatial + (1 - alpha) * x_temporal`)
+// out = a * x + b * y for fp32 a, b with each product and the sum rounded to 16 bits: torch's `a * x + b * y` for Python-float
+// a, b on 16-bit tensors (diffusers AlphaBlender.forward: `alpha * x_spatial + (1 - alpha) * x_temporal`).  The coefficients
+// are used as given: the caller passes sigmoid(mix_factor) in fp32, where the stock 16-bit module rounds alpha to the model
+// dtype first and computes 1 - alpha in that dtype.
 template <bool BF16>
 __global__ void axpby_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, uint4* __restrict__ out, long n16,
                              float a, float b) {
@@ -487,8 +489,10 @@ __global__ void svd_in_assemble_kernel(const void* __restrict__ x, const void* _
 
 // SVD loop, output side (models/pipeline.py:433-439): per-frame classifier-free guidance
 //   v = v_u + g_f (v_c - v_u), g_f = linspace(min, max, F)[f]      (16-bit roundings of every op, as torch does on fp16)
-// then EulerDiscreteScheduler.step with v-prediction in fp32:
+// then EulerDiscreteScheduler.step with v-prediction, all in fp32:
 //   x0 = v * (-sigma / sqrt(sigma^2 + 1)) + x / (sigma^2 + 1);  x' = x + (x - x0) / sigma * (sigma_next - sigma)
+// The product v * (-sigma / ...) is not rounded to 16 bits.  diffusers rounds it when the model output is 16-bit (16-bit tensor
+// times 0-d fp32 tensor); keeping fp32 is what the fp32 pipeline computes.
 // pred: fp32 [2B*F*h*w, ldc] channels-last straight from conv_out (rows: uncond half then cond half); x, x_out [B, F, 4, h, w].
 template <bool BF16>
 __global__ void svd_cfg_euler_step_kernel(const float* __restrict__ pred, int ldc, int cfg, const float* __restrict__ gs,

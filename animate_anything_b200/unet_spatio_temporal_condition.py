@@ -125,7 +125,9 @@ class TransformerSpatioTemporalModel(_ParamsOnly):
 
 # ------------------------------------------------------------------------------------------------ weight preparation
 def _alpha(m: AlphaBlender) -> float:
-    """image_only_indicator is all zeros on this path -> alpha = sigmoid(mix_factor) for both strategies."""
+    """image_only_indicator is all zeros on this path -> alpha = sigmoid(mix_factor) for both strategies.  Kept in fp32 and
+    not rounded to the model dtype (the stock 16-bit AlphaBlender rounds alpha first, then takes 1 - alpha in 16 bits):
+    `aab_axpby` gets alpha and 1 - alpha as fp32 coefficients, as the fp32 reference computes them."""
     a = float(torch.sigmoid(m.mix_factor.detach().float()).item())
     return 1.0 - a if m.switch_spatial_to_temporal_mix else a
 

@@ -38,7 +38,9 @@ int aab_igemm_emits_colstats(const AabIgemmDesc* desc);
  * k, v: columns k_col0 / v_col0 of kv [nb_kv*lk, ldkv]; query batch b reads kv batch b / kv_batch_div.
  * `is_bf16` bit 0: bfloat16 (else float16); bit 1: causal mask (key j visible to query i iff j <= i; needs lq == lk <= 128):
  * the CLIP text tower's self-attention (transformers CLIPAttention + causal_attention_mask), reached from
- * models/pipeline.py:136 `_encode_prompt`. */
+ * models/pipeline.py:136 `_encode_prompt`.
+ * Rejected with 1: col0 + 64 heads past q_cols / kv_cols, (nb - 1) / kv_batch_div >= nb_kv, q / kv / out not 16-byte aligned,
+ * row or batch strides not multiples of 8. */
 int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, int q_cols, int q_col0, const void* kv, long ldkv,
                        long kv_batch_stride, int kv_cols, int k_col0, int v_col0, void* out, long ld_out,
                        long out_batch_stride, int out_col0, int nb, int nb_kv, int kv_batch_div, int heads, int lq, int lk,
@@ -67,7 +69,9 @@ int aab_clip_image_prep(const void* src, int src_type, long sb, long sc, long sy
                         int patch, void* out, long ld_out, int is_bf16, void* stream);
 
 /* Self-attention over the frame axis (T <= 32) without the (b t) c h w -> (b h w) t c permutes
- * (diffusers TransformerTemporalModel.forward; models/unet_3d_blocks.py:299-306,459-467,694-701). */
+ * (diffusers TransformerTemporalModel.forward; models/unet_3d_blocks.py:299-306,459-467,694-701).
+ * qkv rows ((b t) hw, ld); head h of q / k / v at columns col0 + 64 h.  Rejected with 1: t outside 1..32, b, hw or heads < 1,
+ * col0 + 64 heads > ld, 64 heads > ld_out, ld / ld_out / col0 not multiples of 8, qkv / out not 16-byte aligned. */
 int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k_col0, int v_col0, void* out, long ld_out, int b, int t,
                           int hw, int heads, float scale, int is_bf16, void* stream);
 
@@ -111,7 +115,9 @@ int aab_embed_tokens(const long long* ids, const void* tok_emb, const void* pos_
  * 9-channel UNet input [N, C<=16, H, W] -> channels-last padded to 16 (:422 cat([mask, latents, image_latents], dim=2));
  * out[r] = x[r] + vec[idx(r)], out may alias x (single-key cross-attention = per-sample vector; frame position embedding; mode 1 = the
  * (h*w, batch)-ordered time_context quirk of TransformerSpatioTemporalModel.forward);
- * AlphaBlender a*x + b*y with torch's 16-bit roundings; conv_out -> [B, F, 4, H, W]. */
+ * AlphaBlender out = a*x + b*y for fp32 a, b: each product and the sum rounded to 16 bits, as torch computes `a * x + b * y`
+ * for Python-float a, b (the caller passes alpha = sigmoid(mix_factor) in fp32; the stock 16-bit AlphaBlender would first
+ * round alpha to the model dtype); conv_out -> [B, F, 4, H, W]. */
 int aab_image_to_nhwc16(const void* img, long sn, long sc, long sy, long sx, void* out, long n, int c, int h, int w,
                         int is_bf16, void* stream);
 int aab_add_rowvec(const void* x, long ldx, void* out, long ldo, const float* vec, long ldv, long rows, int cols,
@@ -119,7 +125,9 @@ int aab_add_rowvec(const void* x, long ldx, void* out, long ldo, const float* ve
 int aab_axpby(const void* x, const void* y, void* out, long n_elems, float a, float b, int is_bf16, void* stream);
 int aab_svd_out_finalize(const float* y, int ldc, void* out, long bf, int h, int w, int is_bf16, void* stream);
 /* SVD loop boundary kernels (models/pipeline.py:416-439): scale_model_input + CFG duplication + 9-channel cat in one pass;
- * per-frame guidance + Euler step (v-prediction) in one pass.  gs: fp32 [f] = linspace(min, max, f) (:405-408). */
+ * per-frame guidance + Euler step (v-prediction) in one pass.  gs: fp32 [f] = linspace(min, max, f) (:405-408).
+ * Guidance: v = v_u + g (v_c - v_u) with the 16-bit roundings of torch (pred, gs and every op rounded); the Euler step is
+ * then fp32 throughout, including v * (-sigma / sqrt(sigma^2 + 1)), which diffusers would round to 16 bits for a 16-bit v. */
 int aab_svd_in_assemble(const void* x, const void* img_lat, const void* mask, float inv_scale, void* out, int b, int f, int h,
                         int w, int cfg, int is_bf16, void* stream);
 /* General form for TextStableVideoDiffusionPipeline.__call__ (models/pipeline.py:596-606 conditioning latents per frame, either

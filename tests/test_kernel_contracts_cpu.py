@@ -1,0 +1,159 @@
+"""CPU: argument checks of the attention entry points (fake buffers, only calls that return before any launch), the table of
+which GPU test covers each C-ABI entry point of include/aab200.h, and the AlphaBlender coefficient the SVD UNet hands to
+`aab_axpby`."""
+import ctypes as C
+import os
+import re
+
+import pytest
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "aab200.h")
+
+
+# ---------------------------------------------------------------------------------------------- argument checks
+@pytest.fixture(scope="module")
+def buffers():
+    from animate_anything_b200 import _lib
+    lib = _lib.load()
+    buf = (C.c_float * 4096)()
+    p = C.c_void_p((C.addressof(buf) + 15) // 16 * 16)
+    return lib, buf, p
+
+
+def test_flash_attn_d64_rejects_bad_arguments_without_a_gpu(buffers):
+    lib, _, p = buffers
+    mis = C.c_void_p(p.value + 2)
+
+    def fa(q=p, kv=p, out=p, ldq=192, ldkv=192, ld_out=64, q_bs=None, kv_bs=None, q_cols=192, kv_cols=192, q_col0=0,
+           k_col0=64, v_col0=128, out_col0=0, nb=2, nb_kv=2, div=1, heads=1, lq=4, lk=4, bf=0):
+        return lib.aab_flash_attn_d64(q, ldq, lq * ldq if q_bs is None else q_bs, q_cols, q_col0, kv, ldkv,
+                                      lk * ldkv if kv_bs is None else kv_bs, kv_cols, k_col0, v_col0, out, ld_out, lq * ld_out,
+                                      out_col0, nb, nb_kv, div, heads, lq, lk, 0.125, bf, None)
+    assert fa(q=None) == 1 and fa(kv=None) == 1 and fa(out=None) == 1
+    assert fa(lq=0) == 1 and fa(lk=0) == 1 and fa(heads=0) == 1 and fa(nb=0) == 1 and fa(nb_kv=0) == 1 and fa(div=0) == 1
+    assert fa(ldq=196) == 1 and fa(ldkv=196) == 1 and fa(ld_out=68) == 1 and fa(out_col0=4) == 1   # strides / offset % 8
+    assert fa(bf=3, lq=4, lk=8) == 1 and fa(bf=2, lq=129, lk=129) == 1                 # causal: lq == lk <= 128 only
+    # misaligned bases and batch strides (TMA needs 16-byte addresses)
+    assert fa(q=mis) == 1 and fa(kv=mis) == 1 and fa(out=mis) == 1
+    assert fa(q_bs=4 * 192 + 4) == 1 and fa(kv_bs=4 * 192 + 4) == 1
+    # heads outside the described columns: TMA would read zero fill and return wrong attention
+    assert fa(heads=2) == 1                                                          # V: 128 + 2 x 64 > 192 columns
+    assert fa(q_col0=160) == 1 and fa(k_col0=136) == 1 and fa(v_col0=136) == 1
+    assert fa(q_col0=-8) == 1 and fa(k_col0=-8) == 1 and fa(v_col0=-64) == 1
+    assert fa(q_cols=56) == 1 and fa(kv_cols=184) == 1
+    # a query batch whose K/V batch b / kv_batch_div does not exist
+    assert fa(nb=3, nb_kv=2) == 1 and fa(nb=5, nb_kv=2, div=2) == 1 and fa(nb=7, nb_kv=2, div=3) == 1
+
+
+def test_temporal_attn_d64_rejects_bad_arguments_without_a_gpu(buffers):
+    lib, _, p = buffers
+    mis = C.c_void_p(p.value + 8)
+
+    def ta(qkv=p, out=p, ld=384, ld_out=128, q_col0=0, k_col0=128, v_col0=256, b=1, t=4, hw=2, heads=2):
+        return lib.aab_temporal_attn_d64(qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw, heads, 0.125, 0, None)
+    assert ta(qkv=None) == 1 and ta(out=None) == 1
+    assert ta(t=0) == 1 and ta(t=33) == 1
+    assert ta(b=0) == 1 and ta(hw=0) == 1 and ta(heads=0) == 1 and ta(b=-1) == 1
+    assert ta(ld=388) == 1 and ta(ld_out=132) == 1 and ta(k_col0=132) == 1
+    assert ta(qkv=mis) == 1 and ta(out=mis) == 1
+    assert ta(v_col0=320) == 1 and ta(q_col0=264) == 1 and ta(heads=3) == 1          # a head past the end of a qkv row
+    assert ta(ld_out=64) == 1                                                          # output row narrower than heads x 64
+    assert ta(q_col0=-8) == 1
+
+
+# ---------------------------------------------------------------------------------------------- coverage table
+# Every entry point of include/aab200.h -> (GPU test that checks it directly, note).  A test id is "file::function"; a row
+# without one says why there is no direct test.  A new entry point without a row fails test_every_entry_point_has_a_row.
+KC = "test_gpu_kernel_contracts.py"
+AE = "test_gpu_attention_edges.py"
+COVERAGE = {
+    "aab_igemm": ("test_gpu_igemm.py::test_linear_plain", "plus conv / tconv / batched / cluster variants in that file"),
+    "aab_igemm_emits_colstats": ("test_gpu_norm_elem.py::test_igemm_column_statistics", ""),
+    "aab_flash_attn_d64": (f"{AE}::test_flash_d64_tail_lengths", "plus score patterns, leakage, causal, arguments"),
+    "aab_flash_attn_d80": (f"{AE}::test_flash_d80_tail_lengths", "plus test_gpu_clip_vision.py::test_flash_d80_self"),
+    "aab_clip_image_prep": ("test_gpu_clip_vision.py::test_clip_image_prep_matches_restatement", ""),
+    "aab_temporal_attn_d64": (f"{AE}::test_temporal_frame_counts", "plus persistent loop, large logits, v1 == v2"),
+    "aab_groupnorm_workspace_bytes": ("test_gpu_norm_elem.py::test_groupnorm", "host-side size query, used by every GroupNorm"),
+    "aab_groupnorm": ("test_gpu_norm_elem.py::test_groupnorm", ""),
+    "aab_groupnorm_colstats": ("test_gpu_norm_elem.py::test_groupnorm_from_producer_statistics", ""),
+    "aab_layernorm": ("test_gpu_norm_elem.py::test_layernorm", ""),
+    "aab_softmax_rows": ("test_gpu_norm_elem.py::test_softmax_rows_and_transpose", ""),
+    "aab_unet_in_assemble": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_unet_out_finalize": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_timestep_embed": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_embed_tokens": (f"{KC}::test_embed_tokens", ""),
+    "aab_image_to_nhwc16": (f"{KC}::test_image_to_nhwc16", ""),
+    "aab_add_rowvec": (f"{KC}::test_add_rowvec", ""),
+    "aab_axpby": (f"{KC}::test_axpby", ""),
+    "aab_svd_out_finalize": (f"{KC}::test_svd_out_finalize", ""),
+    "aab_svd_in_assemble": (f"{KC}::test_svd_in_assemble", ""),
+    "aab_svd_in_assemble_frames": ("test_gpu_svd.py::test_svd_in_assemble_frames_kernel", ""),
+    "aab_svd_cfg_euler_step": (f"{KC}::test_svd_cfg_euler_step", ""),
+    "aab_geglu": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_upsample2x": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_upsample_nearest": (f"{KC}::test_upsample_nearest_unet_sizes", "plus test_upsample_nearest_sweep"),
+    "aab_pad_br": (f"{KC}::test_pad_to_even", ""),
+    "aab_copy2d": (f"{KC}::test_copy2d_both_paths", ""),
+    "aab_dup_rows": (f"{KC}::test_dup_rows", ""),
+    "aab_transpose": ("test_gpu_norm_elem.py::test_softmax_rows_and_transpose", ""),
+    "aab_cfg_scheduler_step": ("test_gpu_norm_elem.py::test_cfg_scheduler_step", ""),
+    "aab_image_to_nhwc8": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
+    "aab_vae_enc_finalize": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
+    "aab_vae_dec_in": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
+    "aab_vae_dec_finalize": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
+    "aab_vae_dec_finalize_u8": ("test_gpu_transparent.py::test_masked_latent_to_video_pipeline",
+                                "end to end only: the uint8 frames of the transparent-video pipeline against the reference"),
+    "aab_add_noise": ("test_gpu_pipeline.py::test_common_ddpm_forward_timesteps_bit_exact", ""),
+    "aab_video_f32_to_nhwc8": ("test_gpu_transparent.py::test_video_f32_to_nhwc8_and_rgba_finalize_bit_exact", ""),
+    "aab_rgba_finalize_u8": ("test_gpu_transparent.py::test_video_f32_to_nhwc8_and_rgba_finalize_bit_exact", ""),
+    "aab_pad_cols": ("test_gpu_transparent.py::test_pad_cols_and_cat_cols", ""),
+    "aab_cast_f32": (f"{KC}::test_cast_f32_special_values", "no caller in the package; tested so that it can be used"),
+    "aab_num_sms": (None, "host query of the device's SM count, no kernel: nothing to compare"),
+}
+
+
+def _header_entry_points():
+    text = open(HEADER).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    return re.findall(r"^\s*(?:int|long)\s+(aab_\w+)\s*\(", text, flags=re.M)
+
+
+def test_every_entry_point_has_a_row():
+    names = _header_entry_points()
+    assert len(names) == len(set(names)) and len(names) >= 40, names
+    missing = sorted(set(names) - set(COVERAGE))
+    stale = sorted(set(COVERAGE) - set(names))
+    assert not missing, f"entry points without a row in COVERAGE: {missing}"
+    assert not stale, f"rows for entry points the header no longer declares: {stale}"
+
+
+@pytest.mark.parametrize("name", sorted(COVERAGE))
+def test_coverage_row_names_a_gpu_test_or_a_reason(name):
+    test_id, note = COVERAGE[name]
+    if test_id is None:
+        assert note, f"{name}: no test and no reason"
+        return
+    fname, func = test_id.split("::")
+    src = open(os.path.join(ROOT, "tests", fname)).read()
+    m = re.search(rf"^def {func}\(", src, flags=re.M)
+    assert m, f"{name}: {test_id} does not exist"
+    # the test (or its module) runs under -m gpu
+    head = src[:m.start()].rsplit("\ndef ", 1)[-1]
+    assert "pytestmark = pytest.mark.gpu" in src or "@pytest.mark.gpu" in head, f"{test_id} is not a GPU test"
+
+
+# ---------------------------------------------------------------------------------------------- AlphaBlender coefficient
+@pytest.mark.parametrize("mix", [0.5, -0.37, 1.3])
+@pytest.mark.parametrize("switch", [False, True])
+def test_alpha_blender_coefficient_is_fp32_sigmoid(mix, switch):
+    """The SVD UNet passes alpha = sigmoid(mix_factor) in fp32 (not rounded to the model dtype) to `aab_axpby`; the other
+    coefficient is 1 - alpha.  tests/test_gpu_kernel_contracts.py::test_axpby pins the kernel's roundings for such
+    coefficients."""
+    from animate_anything_b200.unet_spatio_temporal_condition import AlphaBlender, _alpha
+    m = AlphaBlender(mix, "learned_with_images", switch_spatial_to_temporal_mix=switch)
+    s = float(torch.sigmoid(torch.tensor(mix, dtype=torch.float32)).item())
+    assert _alpha(m) == (1.0 - s if switch else s)
+    for dt in (torch.float16, torch.bfloat16):
+        assert s != float(torch.tensor(s).to(dt))                  # the 16-bit-rounded alpha would be a different value
