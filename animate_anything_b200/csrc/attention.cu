@@ -544,15 +544,6 @@ temporal_attn_d64_kernel(const void* __restrict__ qkv, long ld, int q_col0, int 
 // the Q/K/V rows of the NEXT item are fetched with 16-byte cp.async copies straight into the second shared-memory buffer
 // (408 copies in flight per warp, no registers involved) while the current item is computed; the normalised output is
 // staged in shared memory and written with 16-byte stores (one 128-byte row per 8 lanes).
-__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gmem_src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
 template <bool BF16>
 __global__ void __launch_bounds__(128)
 temporal_attn_d64_v2_kernel(const void* __restrict__ qkv, long ld, int q_col0, int k_col0, int v_col0,

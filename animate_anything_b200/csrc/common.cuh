@@ -134,6 +134,16 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// ---------------------------------------------------------------- cp.async (16-byte global -> shared copies, no registers)
+__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
 // ---------------------------------------------------------------- thread-block clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

@@ -17,9 +17,13 @@
 //   n-tile; each fetches 1/cluster of the weight tile and multicasts it to all of them, so a k-block reads the weights from
 //   L2 once per cluster instead of once per CTA.  A stage is refilled only after the consumers of every CTA of the cluster
 //   have released it.  Same K order, same epilogue: bit-identical to single CTAs.
-// * Epilogue straight from the accumulator registers: bias / per-sample bias (time embedding) / residual / activation
-//   / GEGLU gate -> 16-bit (or fp32) stores, masked at the tile edges, plus optional per-tile column statistics for the
-//   GroupNorm that follows.
+// * Tile widths 32 / 64 / 128 / 160 / 192 / 256: the caller fits the width to N and to the number of tiles per wave, because
+//   a ragged last N tile costs no traffic (TMA zero-fill) but issues every wgmma of its dead columns.
+// * Epilogue: bias / per-sample bias (time embedding) / residual / activation / GEGLU gate, masked at the tile edges, plus
+//   optional per-tile column statistics for the GroupNorm that follows.  16-bit outputs are transposed through a per-warp
+//   shared-memory slab so that the residual comes in and the result leaves as 16-byte accesses of whole 64-byte row
+//   segments (the accumulator layout alone gives 4-byte accesses, half a sector per row); the stores are not waited for, so
+//   they drain under the next tile's main loop.  fp32 / odd-N / scaled outputs are stored per element from the registers.
 //
 // Replaces, for the reference path (SURVEY.md section 8a): cuDNN conv2d/conv3d and cuBLAS linear calls made by
 // diffusers ResnetBlock2D / TemporalConvLayer / Transformer2DModel / TransformerTemporalModel / AutoencoderKL
@@ -37,15 +41,22 @@ constexpr int NUM_CONSUMERS = 2;                 // consumer warpgroups, 64 tile
 constexpr int NUM_THREADS = 128 * (1 + NUM_CONSUMERS);
 constexpr int NUM_CONSUMER_WARPS = 4 * NUM_CONSUMERS;
 
-// smem ring depth per tile width: 192 KiB (160 KiB for BN = 32) of operands in flight whatever BN, plus the column-statistics
-// scratch, inside the 227 KiB a block may use
+// staged epilogue: every consumer warp owns two slabs (used in turn) of its 16 tile rows x 32 columns: 64-byte rows, 16-byte
+// chunks XOR-swizzled by the row pair so that neither the accumulator-layout word accesses nor the 16-byte row accesses
+// conflict on a bank
+constexpr int SLAB_COLS = 32;
+constexpr int SLAB_BYTES = 16 * SLAB_COLS * 2;   // 1 KiB
+
+// smem ring depth per tile width: 160 - 200 KiB of operands in flight whatever BN, plus the column-statistics scratch and the
+// epilogue slabs, inside the 227 KiB a block may use
 template <int BN>
 struct Cfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
+  static constexpr int STAGES = (BN >= 192) ? 4 : (BN == 160) ? 5 : (BN == 128) ? 6 : 8;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STATS_BYTES = NUM_CONSUMER_WARPS * BN * 2 * 4;   // per-warp (sum, sum of squares) per column
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + STATS_BYTES + 1024 /*align*/ +
-                                    256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + STATS_BYTES +
+                                    NUM_CONSUMER_WARPS * 2 * SLAB_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "tile configuration exceeds the shared memory of an SM");
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -68,8 +79,9 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_addr, uint32_t
 
 // GEGLU: B tile = [values | gates] (BN/2 rows each), out = value * gelu(gate), BN/2 columns.
 // Epilogue flavours (runtime, uniform per launch):
-//   staged  (no AAB_F_DIRECT): n_out % 32 == 0, 16-bit output, at most one of residual / per-sample bias / SiLU, no scaling;
-//                              column pairs are stored as 32-bit words; may emit column statistics
+//   staged  (no AAB_F_DIRECT): n_out % 32 == 0, 16-bit output, 16-byte aligned rows, at most one of residual / per-sample
+//                              bias / SiLU, no scaling; goes through the warp's shared-memory slab and leaves as 16-byte
+//                              stores of whole 64-byte row segments; may emit column statistics
 //   direct  (AAB_F_DIRECT):    any n_out, fp32 or 16-bit output, every flag combination, masked per element
 template <int BN, bool GEGLU, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -84,7 +96,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   uint8_t* smA = smem;
   uint8_t* smB = smA + STAGES * A_STAGE_BYTES;
   float* sstats = reinterpret_cast<float*>(smB + STAGES * CF::B_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sstats) + CF::STATS_BYTES);
+  uint8_t* slabs = reinterpret_cast<uint8_t*>(sstats) + CF::STATS_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(slabs + NUM_CONSUMER_WARPS * 2 * SLAB_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
 
@@ -246,79 +259,133 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       grow[h] = ((static_cast<long>(g[3]) * p.dimD[2] + g[2]) * p.dimD[1] + g[1]) * p.dimD[0] + g[0];
     }
     const int n0 = nt * OUT_BN;
-    const float* bias2row[2];
-    const uint8_t* resrow[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      bias2row[h] = (p.bias2 != nullptr && rvalid[h]) ? p.bias2 + (grow[h] / p.rows_per_bias2) * p.ld_bias2 : nullptr;
-      resrow[h] = (p.residual != nullptr && rvalid[h])
-                      ? reinterpret_cast<const uint8_t*>(p.residual) + grow[h] * p.ld_res * 2
-                      : nullptr;
-    }
+    // per-sample bias row and residual row of a valid accumulator row (formed where used: pointers kept across the
+    // epilogue would not fit beside a 256-column accumulator)
+    auto bias2row = [&](int h) { return p.bias2 + (grow[h] / p.rows_per_bias2) * p.ld_bias2; };
+    auto resrow = [&](int h) { return reinterpret_cast<const uint8_t*>(p.residual) + grow[h] * p.ld_res * 2; };
+    const bool has_bias2 = p.bias2 != nullptr;
     if (stats) named_bar_sync(1, 128 * NUM_CONSUMERS);     // the previous tile's statistics scratch has been read
 
+    if (GEGLU || !direct) {
+      if constexpr (BN >= 64) {
+        // ---- staged: the warp converts 32 columns of its 16 rows at a time into its slab, then the slab leaves as 16-byte
+        // pieces of whole 64-byte row segments.  In both views of the slab a thread owns rows (lane >> 2) and (lane >> 2) + 8:
+        // as words of chunk j (accumulator layout, columns 8 j + 2 (lane & 3)) and as the whole chunk (lane & 3).  The
+        // residual takes the same way in.  Global stores are not waited for: the warp is back in the main loop of its next
+        // tile while they drain.
+        const int q = lane & 3;
+        const int sw = (lane >> 3) & 3;                        // chunk swizzle of both rows (row pair index mod 4)
+        uint8_t* const srow0 = slabs + (cw * 4 + wq) * 2 * SLAB_BYTES + (lane >> 2) * (SLAB_COLS * 2);
+        constexpr int H_OFF = 8 * SLAB_COLS * 2;               // row r + 8 of the slab
+        const int vec_off = (q ^ sw) << 4;
+        const int nslab = (min(OUT_BN, p.n_out - n0)) / SLAB_COLS;   // n_out is a multiple of 32
+        const bool has_res = !GEGLU && p.residual != nullptr;
+        auto fetch_res = [&](int s) {                          // residual of slab s -> slab buffer s & 1, no registers held
 #pragma unroll
-    for (int jj = 0; jj < OUT_BN / 8; ++jj) {
-      const int cl = jj * 8 + 2 * (lane & 3);                // tile column of this thread's pair
-      const int col = n0 + cl;
-      float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
+          for (int h = 0; h < 2; ++h)
+            if (rvalid[h])
+              cp_async_16(srow0 + (s & 1) * SLAB_BYTES + h * H_OFF + vec_off, resrow(h) + (n0 + s * SLAB_COLS + 8 * q) * 2);
+          cp_async_commit();
+        };
+        __syncwarp();                                          // the previous tile's last slab has been read
+        if (has_res) fetch_res(0);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float x[2] = {acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]};
-        if (GEGLU) {
-          float g[2] = {acc[4 * (jj + BN / 16) + 2 * h], acc[4 * (jj + BN / 16) + 2 * h + 1]};
-          if (col < p.n_out) {
-            if (p.bias != nullptr) {
-              const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-              const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
-              x[0] += bv.x; x[1] += bv.y;
-              g[0] += bg.x; g[1] += bg.y;
+        for (int s = 0; s < OUT_BN / SLAB_COLS; ++s) {
+          if (s >= nslab) break;                               // warp-uniform: a ragged last n-tile
+          uint8_t* const sb = srow0 + (s & 1) * SLAB_BYTES;
+          if (has_res) cp_async_wait<0>();
+          __syncwarp();                                        // this slab's residual has landed; the other buffer has been read
+          if (has_res && s + 1 < nslab) fetch_res(s + 1);      // in flight while this slab is converted
+#pragma unroll
+          for (int j = 0; j < SLAB_COLS / 8; ++j) {
+            const int jj = s * (SLAB_COLS / 8) + j;
+            const int cl = jj * 8 + 2 * q;                     // tile column of this thread's pair
+            const int col = n0 + cl;
+            const int word_off = ((j ^ sw) << 4) + q * 4;
+            float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float x[2] = {acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]};
+              uint32_t* wp = reinterpret_cast<uint32_t*>(sb + h * H_OFF + word_off);
+              if (GEGLU) {
+                float g[2] = {acc[4 * (jj + BN / 16) + 2 * h], acc[4 * (jj + BN / 16) + 2 * h + 1]};
+                if (p.bias != nullptr) {
+                  const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                  const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
+                  x[0] += bv.x; x[1] += bv.y;
+                  g[0] += bg.x; g[1] += bg.y;
+                }
+                *wp = pack2(x[0] * gelu_fast_f(g[0]), x[1] * gelu_fast_f(g[1]), bf16);
+              } else {
+                if (p.bias != nullptr) {
+                  const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                  x[0] += b.x; x[1] += b.y;
+                }
+                if (has_bias2 && rvalid[h]) {
+                  const float2 b = __ldg(reinterpret_cast<const float2*>(bias2row(h) + col));
+                  x[0] += b.x; x[1] += b.y;
+                }
+                if (has_res) {
+                  const float2 r = unpack2(*wp, bf16);
+                  x[0] += r.x; x[1] += r.y;
+                }
+                if (p.act == AAB_ACT_SILU) {
+                  x[0] = silu_fast_f(x[0]);
+                  x[1] = silu_fast_f(x[1]);
+                }
+                const uint32_t o = pack2(x[0], x[1], bf16);
+                *wp = o;
+                if (stats && rvalid[h]) {
+                  const float2 f = unpack2(o, bf16);           // statistics of the ROUNDED 16-bit outputs
+                  ssum[0] += f.x; ssq[0] = fmaf(f.x, f.x, ssq[0]);
+                  ssum[1] += f.y; ssq[1] = fmaf(f.y, f.y, ssq[1]);
+                }
+              }
             }
-            if (rvalid[h]) {
-              const uint32_t o = pack2(x[0] * gelu_fast_f(g[0]), x[1] * gelu_fast_f(g[1]), bf16);
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(p.out) + (grow[h] * p.ld_out + col) * 2) = o;
-            }
-          }
-        } else if (!direct) {
-          if (col < p.n_out) {
-            if (p.bias != nullptr) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-              x[0] += b.x; x[1] += b.y;
-            }
-            if (bias2row[h] != nullptr) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(bias2row[h] + col));
-              x[0] += b.x; x[1] += b.y;
-            }
-            if (resrow[h] != nullptr) {
-              const float2 r = unpack2(__ldg(reinterpret_cast<const unsigned int*>(resrow[h] + col * 2)), bf16);
-              x[0] += r.x; x[1] += r.y;
-            }
-            if (p.act == AAB_ACT_SILU) {
-              x[0] = silu_fast_f(x[0]);
-              x[1] = silu_fast_f(x[1]);
-            }
-            const uint32_t o = pack2(x[0], x[1], bf16);
-            if (rvalid[h]) {
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(p.out) + (grow[h] * p.ld_out + col) * 2) = o;
-              if (stats) {
-                const float2 f = unpack2(o, bf16);           // statistics of the ROUNDED 16-bit outputs
-                ssum[0] += f.x; ssq[0] = fmaf(f.x, f.x, ssq[0]);
-                ssum[1] += f.y; ssq[1] = fmaf(f.y, f.y, ssq[1]);
+            if (stats) {
+              // sum over the warp's 16 rows: the 8 lanes sharing (lane & 3) hold this column pair; fixed-order butterfly
+#pragma unroll
+              for (int off = 4; off < 32; off <<= 1) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  ssum[e] += __shfl_xor_sync(0xffffffffu, ssum[e], off);
+                  ssq[e] += __shfl_xor_sync(0xffffffffu, ssq[e], off);
+                }
+              }
+              if (lane < 4) {
+                float* sp = sstats + ((cw * 4 + wq) * BN + cl) * 2;
+                sp[0] = ssum[0]; sp[1] = ssq[0]; sp[2] = ssum[1]; sp[3] = ssq[1];
               }
             }
           }
-        } else {
+          __syncwarp();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (rvalid[h])
+              *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) +
+                                        (grow[h] * p.ld_out + n0 + s * SLAB_COLS + 8 * q) * 2) =
+                  *reinterpret_cast<const uint4*>(sb + h * H_OFF + vec_off);
+          }
+        }
+      }
+    } else if constexpr (!GEGLU) {
+      // ---- direct: masked per element, straight from the accumulator registers
+#pragma unroll
+      for (int jj = 0; jj < OUT_BN / 8; ++jj) {
+        const int col = n0 + jj * 8 + 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             if (col + e < p.n_out) {
-              float v = x[e];
+              float v = acc[4 * jj + 2 * h + e];
               if (p.bias != nullptr) v += __ldg(p.bias + col + e);
-              if (bias2row[h] != nullptr) v += __ldg(bias2row[h] + col + e);
+              if (has_bias2 && rvalid[h]) v += __ldg(bias2row(h) + col + e);
               if (scale_acc) {
                 v = apply_act(v, p.act) * p.out_scale;
-                if (resrow[h] != nullptr) v += load_elem(resrow[h], col + e, bf16);
+                if (p.residual != nullptr && rvalid[h]) v += load_elem(resrow(h), col + e, bf16);
               } else {
-                if (resrow[h] != nullptr) v += load_elem(resrow[h], col + e, bf16);
+                if (p.residual != nullptr && rvalid[h]) v += load_elem(resrow(h), col + e, bf16);
                 v = apply_act(v, p.act) * p.out_scale;
               }
               if (rvalid[h]) {
@@ -327,21 +394,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               }
             }
           }
-        }
-      }
-      if (stats) {
-        // sum over the warp's 16 rows: the 8 lanes sharing (lane & 3) hold this column pair; fixed-order butterfly
-#pragma unroll
-        for (int off = 4; off < 32; off <<= 1) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            ssum[e] += __shfl_xor_sync(0xffffffffu, ssum[e], off);
-            ssq[e] += __shfl_xor_sync(0xffffffffu, ssq[e], off);
-          }
-        }
-        if (lane < 4) {
-          float* sp = sstats + ((cw * 4 + wq) * BN + cl) * 2;
-          sp[0] = ssum[0]; sp[1] = ssq[0]; sp[2] = ssum[1]; sp[3] = ssq[1];
         }
       }
     }
@@ -489,7 +541,8 @@ static int igemm_is_staged(const AabIgemmDesc* d) {
   const int bn = d->block_n;
   const int n_out = geglu ? d->n / 2 : d->n;
   if ((d->flags & (AAB_F_DIRECT | AAB_F_OUT_F32 | AAB_F_SCALE_ACC)) || bn == 32 || (d->ld_out % 8) || (n_out % 32)) return 0;
-  if (d->residual && (d->ld_res % 8)) return 0;
+  if (reinterpret_cast<uintptr_t>(d->out) % 16) return 0;   // rows are stored and the residual is read 16 bytes at a time
+  if (d->residual && ((d->ld_res % 8) || reinterpret_cast<uintptr_t>(d->residual) % 16)) return 0;
   if ((d->act == AAB_ACT_GELU || d->act == AAB_ACT_QUICK_GELU) && !geglu) return 0;
   const int extras = (d->residual ? 1 : 0) + (d->bias2 ? 1 : 0) + (d->act == AAB_ACT_SILU ? 1 : 0);
   if (!geglu && (extras > 1 || d->out_scale != 1.0f)) return 0;
@@ -506,18 +559,13 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
   const int is_bf16 = (d->flags & AAB_F_BF16) ? 1 : 0;
   const bool geglu = (d->flags & AAB_F_GEGLU) != 0;
   int bn = d->block_n;
-  if (bn != 32 && bn != 64 && bn != 128 && bn != 256) return AAB_ERR_ARG;
-  bool direct = (d->flags & AAB_F_DIRECT) != 0;
+  if (bn != 32 && bn != 64 && bn != 128 && bn != 160 && bn != 192 && bn != 256) return AAB_ERR_ARG;
   const int n_out = geglu ? d->n / 2 : d->n;
-  if (bn == 32 || (d->ld_out % 8) != 0 || (n_out % 32) != 0 || (d->flags & AAB_F_OUT_F32)) direct = true;
-  if (geglu && (bn < 128 || direct)) return AAB_ERR_ARG;   // the gate half of the tile must be a whole number of 64-column blocks
-  if (d->residual && (d->ld_res % 8) != 0 && !direct) direct = true;
-  if (d->flags & AAB_F_SCALE_ACC) direct = true;
-  if ((d->act == AAB_ACT_GELU || d->act == AAB_ACT_QUICK_GELU) && !geglu) direct = true;
-  {   // the staged epilogue covers one extra term (residual | per-sample bias | SiLU) and no output scaling
-    const int extras = (d->residual ? 1 : 0) + (d->bias2 ? 1 : 0) + (d->act == AAB_ACT_SILU ? 1 : 0);
-    if (!geglu && (extras > 1 || d->out_scale != 1.0f)) direct = true;
-    if (geglu && (extras > 0 || d->out_scale != 1.0f)) return AAB_ERR_ARG;
+  // staged: one extra term (residual | per-sample bias | SiLU), no output scaling, 16-bit rows that can move 16 bytes at a time
+  const bool direct = !igemm_is_staged(d);
+  if (geglu) {   // the gate half of the tile must be a whole number of 64-column blocks; GEGLU only has the staged epilogue
+    if ((bn != 128 && bn != 256) || direct || d->residual || d->bias2 || d->act == AAB_ACT_SILU || d->out_scale != 1.0f)
+      return AAB_ERR_ARG;
   }
   if (d->num_taps < 1 || d->num_taps > AAB_MAX_TAPS) return AAB_ERR_ARG;
   if (d->kc % 8 != 0) return AAB_ERR_ARG;
@@ -591,6 +639,8 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
     case 32: return launch_bn<32, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
     case 64: return launch_bn<64, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
     case 128: return launch_bn<128, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    case 160: return launch_bn<160, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    case 192: return launch_bn<192, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
     default: return launch_bn<256, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
   }
 }

@@ -52,7 +52,7 @@ typedef struct AabIgemmDesc {
   float out_scale;
   int act;
   int flags;
-  int block_n;              // 32 / 64 / 128 / 256
+  int block_n;              // 32 / 64 / 128 / 160 / 192 / 256 (GEGLU: 128 / 256)
   int max_ctas;             // 0 = one CTA per SM
   float* colstats;          // optional [num_m_tiles][n_out][2] fp32: per m-tile column sums (sum, sum of squares) of the ROUNDED
                             // 16-bit outputs over the tile's valid rows -- the statistics of the GroupNorm that follows, taken

@@ -104,9 +104,10 @@ N64_NARROW = os.environ.get("AAB_IGEMM_N64_NARROW", "1") != "0"
 
 
 def pick_block_n(n_out: int, m_tiles: int, geglu: bool = False, k_total: int = 1 << 30) -> int:
-    """Tile width (GEMM columns, multiple of 32, <= 256).  The widest tile wins wherever the main loop dominates: every
+    """Widest tile allowed (GEMM columns: 32 / 64 / 128 / 256).  Wide tiles win wherever the main loop dominates: every
     k-block loads the same 16 KiB of activations whatever the width, so a wide tile reads A once for more columns.  A ragged
-    last N tile costs no traffic (TMA zero-fill beyond N)."""
+    last N tile costs no traffic (TMA zero-fill beyond N) but issues every MMA of its dead columns, so `igemm` narrows a
+    256-column answer to the width that fits N and the wave count (`fit_block_n`)."""
     if geglu:
         return 256 if n_out > 64 else 128
     if m_tiles <= 2:
@@ -120,6 +121,19 @@ def pick_block_n(n_out: int, m_tiles: int, geglu: bool = False, k_total: int = 1
         # epilogue/HBM-bound (tiny K): more tiles than SMs keep every SM busy
         return 128 if m_tiles * -(-n_out // 128) >= NUM_SMS else 64
     return 256
+
+
+def fit_block_n(n_out: int, m_tiles: int, sms: int = NUM_SMS) -> int:
+    """Width actually launched where up to 256 columns are allowed.  All tiles of a launch have one width w and the launch
+    takes ceil(tiles / SMs) waves of w columns each, dead columns of a ragged last tile included: minimise waves * w over
+    128 / 160 / 192 / 256.  Costs within 5 % of the minimum tie and the widest wins a tie (fewer A re-reads per flop).
+    N <= 256 is one n-tile today and stays so.  The K order of an output element does not depend on the width, so
+    results are bit-identical whichever is chosen."""
+    if n_out <= 256:
+        return 256
+    cost = {w: -(-(m_tiles * -(-n_out // w)) // sms) * w for w in (128, 160, 192, 256)}
+    best = min(cost.values())
+    return max(w for w, c in cost.items() if c <= 1.05 * best)
 
 
 def _fix_strides(dims, strides):
@@ -216,6 +230,8 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         flags |= F_PAIR
         if IGEMM_QUAD:
             flags |= F_QUAD
+    elif block_n == 256 and not geglu:
+        block_n = fit_block_n(n_out, m_tiles, _lib.load().aab_num_sms())
     d.flags = flags
     d.block_n = block_n
     d.max_ctas = max_ctas
@@ -236,7 +252,7 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         _lib.call("aab_igemm", C.byref(d), _stream())
         ev1.record()
         IGEMM_PROFILE.append({"rows": rows, "n": n, "k": kc * len(taps), "taps": len(taps), "block_n": block_n,
-                              "pair": bool(flags & F_PAIR),
+                              "pair": bool(flags & F_PAIR), "geglu": geglu, "residual": residual is not None,
                               "flops": 2.0 * rows * n * kc * len(taps), "ev": (ev0, ev1)})
     else:
         _lib.call("aab_igemm", C.byref(d), _stream())
