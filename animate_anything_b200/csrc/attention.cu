@@ -16,7 +16,8 @@
 //    (models/unet_3d_blocks.py:299-306,459-467,694-701; called without encoder_hidden_states so both attn1 and attn2
 //    are self-attention over T).  Activations stay in [B, T, H*W, C] order; the kernel gathers the T rows of one
 //    (b, position, head) with stride H*W*ld, so no permute to [B*H*W, T, C] is ever materialised.  0.1 % of the
-//    FLOPs: CUDA cores, one warp per (position, head).
+//    FLOPs: CUDA cores, one warp per (position, head).  Bit 1 of is_bf16 selects the long-clip kernel (T <= 128): one
+//    4-warp CTA per (b, position, head), 16-query m-tiles per warp, the full score row in registers.
 #include "common.cuh"
 #include "igemm.h"
 #include "wgmma.cuh"
@@ -721,6 +722,185 @@ temporal_attn_d64_v2_kernel(const void* __restrict__ qkv, long ld, int q_col0, i
   cp_async_wait<0>();
 }
 
+// ------------------------------------------------------------------------------------------------ temporal, long clips
+// T in 1..128 (selected by bit 1 of is_bf16).  Persistent CTAs of 4 warps take one (b, pixel, head) item at a time: all 128
+// threads gather its Q/K/V rows with 16-byte cp.async into one of two shared-memory buffers ([3][TP][72] halves, the v2 row
+// stride) while the other buffer is computed.  Warp w owns the 16-query m-tiles w, w + 4 (tiles at or past T are skipped).
+// A 16-query tile's whole score row (TP <= 128 keys = 16 n-tiles x 4 fp32 per lane) stays in registers, so the softmax is
+// one pass over the full row (exp2, scale * log2e, keys >= T at -inf) with no online rescaling; P is packed to 16 bits in
+// registers as the A operand of P.V and the output is normalised once.  Q and K/V fragments come from ldmatrix (.trans for
+// V); key n-tiles / k-steps at or past T are skipped.  The output is staged in the warp's own Q rows and written as 16-byte
+// row stores.  TP = 64 (33..64 frames: 54 KiB, 4 CTAs per SM) or 128 (108 KiB, 2 CTAs per SM).
+constexpr int TAL_THREADS = 128;
+
+__device__ __forceinline__ void ldsm_x4(uint32_t* r, const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t* r, const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
+}
+
+template <int TP>
+constexpr int tal_smem_bytes() { return 2 * 3 * TP * TA_ROW * 2; }
+
+template <bool BF16, int TP>
+__global__ void __launch_bounds__(TAL_THREADS, TP == 64 ? 4 : 2)
+temporal_attn_d64_long_kernel(const void* __restrict__ qkv, long ld, int q_col0, int k_col0, int v_col0,
+                              void* __restrict__ out, long ld_out, int B, int T, int HW, int heads, float scale) {
+  constexpr int NT = TP / 8;          // key n-tiles of S
+  constexpr int KS = TP / 16;         // key k-steps of P.V
+  constexpr int BUF = 3 * TP * TA_ROW;
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ uint16_t sm16[];
+  const int w = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const long total = static_cast<long>(B) * HW * heads;
+  // rows >= T of K and V stay zero for the whole kernel (cp.async only writes rows < T): P.V reads V rows up to the next
+  // multiple of 16, and 0 x (stale bits) could be NaN
+  for (int i = threadIdx.x; i < 2 * BUF / 8; i += TAL_THREADS) reinterpret_cast<uint4*>(sm16)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  auto prefetch = [&](long it, int buf) {
+    const int head = static_cast<int>(it % heads);
+    const long bp = it / heads;
+    const int pos = static_cast<int>(bp % HW);
+    const int b = static_cast<int>(bp / HW);
+    uint16_t* dst = sm16 + buf * BUF;
+    const int nchunks = T * 24;                 // T rows x 3 tensors x 8 pieces of 16 bytes
+    for (int c = threadIdx.x; c < nchunks; c += TAL_THREADS) {
+      const int t = c / 24;
+      const int rem = c - t * 24;
+      const int seg = rem >> 3;
+      const int part = rem & 7;
+      const int col = seg == 0 ? q_col0 : (seg == 1 ? k_col0 : v_col0);
+      const uint8_t* src = reinterpret_cast<const uint8_t*>(qkv) +
+                           (((static_cast<long>(b) * T + t) * HW + pos) * ld + col + head * 64 + part * 8) * 2;
+      cp_async_16(dst + (seg * TP + t) * TA_ROW + part * 8, src);
+    }
+  };
+  long item = blockIdx.x;
+  if (item < total) prefetch(item, 0);
+  cp_async_commit();
+  const int g = lane >> 2;
+  const int t4 = lane & 3;
+  const float sl2 = scale * 1.4426950408889634f;
+  for (int buf = 0; item < total; item += gridDim.x, buf ^= 1) {
+    const long nxt = item + gridDim.x;
+    if (nxt < total) prefetch(nxt, buf ^ 1);    // buf ^ 1 was released by the __syncthreads ending the last round
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();                            // every thread's pieces of this item have landed
+    uint16_t* sQ = sm16 + buf * BUF;
+    const uint16_t* sK = sQ + TP * TA_ROW;
+    const uint16_t* sV = sK + TP * TA_ROW;
+    const int head = static_cast<int>(item % heads);
+    const long bp = item / heads;
+    const int pos = static_cast<int>(bp % HW);
+    const int b = static_cast<int>(bp / HW);
+#pragma unroll 1
+    for (int mt = w; mt * 16 < T; mt += 4) {
+      // ---------------- S = Q K^T for query rows 16 mt .. 16 mt + 15
+      uint32_t afr[4][4];                       // Q A fragments of the four 16-dim k-steps
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) ldsm_x4(afr[kk], sQ + (16 * mt + (lane & 15)) * TA_ROW + 16 * kk + 8 * (lane >> 4));
+      float S[NT][4];
+#pragma unroll
+      for (int nj = 0; nj < NT; ++nj) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) S[nj][e] = 0.f;
+        if (8 * nj < T) {
+          // K rows 8 nj .. 8 nj + 7: matrices at dims 0, 8, 16, 24 (k-steps 0, 1) and 32 .. 56 (k-steps 2, 3)
+          uint32_t kb[8];
+          const uint16_t* kp = sK + (8 * nj + (lane & 7)) * TA_ROW + 8 * (lane >> 3);
+          ldsm_x4(kb, kp);
+          ldsm_x4(kb + 4, kp + 32);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) mma_16816<BF16>(S[nj], afr[kk], kb + 2 * kk);
+        }
+      }
+      // ---------------- softmax over the whole key row: rows g (h = 0) and g + 8 (h = 1)
+      float inv_l[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int nj = 0; nj < NT; ++nj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * nj + 2 * t4 + e;
+            float v = S[nj][2 * h + e] * sl2;
+            v = (col < T) ? v : -INFINITY;
+            S[nj][2 * h + e] = v;
+            mx = fmaxf(mx, v);
+          }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        float l = 0.f;
+#pragma unroll
+        for (int nj = 0; nj < NT; ++nj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float pv = fast_exp2(S[nj][2 * h + e] - mx);
+            S[nj][2 * h + e] = pv;
+            l += pv;
+          }
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv_l[h] = 1.0f / l;
+      }
+      // ---------------- O = P V, P packed from the S registers one 16-key k-step at a time
+      float O[8][4];
+#pragma unroll
+      for (int dj = 0; dj < 8; ++dj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) O[dj][e] = 0.f;
+#pragma unroll
+      for (int k2 = 0; k2 < KS; ++k2) {
+        if (16 * k2 < T) {
+          uint32_t pfr[4];
+          pfr[0] = pack2(S[2 * k2][0], S[2 * k2][1], BF16);
+          pfr[1] = pack2(S[2 * k2][2], S[2 * k2][3], BF16);
+          pfr[2] = pack2(S[2 * k2 + 1][0], S[2 * k2 + 1][1], BF16);
+          pfr[3] = pack2(S[2 * k2 + 1][2], S[2 * k2 + 1][3], BF16);
+          // V rows 16 k2 .. 16 k2 + 15, transposed: matrices (keys +0, dims 8 dj), (+8, 8 dj), (+0, 8 dj + 8), (+8, 8 dj + 8)
+          const uint16_t* vp = sV + (16 * k2 + (lane & 7) + 8 * ((lane >> 3) & 1)) * TA_ROW + 8 * (lane >> 4);
+#pragma unroll
+          for (int dj = 0; dj < 8; dj += 2) {
+            uint32_t vb[4];
+            ldsm_x4_t(vb, vp + 8 * dj);
+            mma_16816<BF16>(O[dj], pfr, vb);
+            mma_16816<BF16>(O[dj + 1], pfr, vb + 2);
+          }
+        }
+      }
+      // ---------------- normalise -> stage in this tile's own Q rows (only this warp reads them) -> 16-byte row stores
+      __syncwarp();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint16_t* orow = sQ + (16 * mt + g + 8 * h) * TA_ROW + 2 * t4;
+#pragma unroll
+        for (int dj = 0; dj < 8; ++dj)
+          *reinterpret_cast<uint32_t*>(orow + dj * 8) = pack2(O[dj][2 * h] * inv_l[h], O[dj][2 * h + 1] * inv_l[h], BF16);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int c = lane; c < 16 * 8; c += 32) {
+        const int t = 16 * mt + (c >> 3);
+        const int part = c & 7;
+        if (t < T) {
+          const uint4 v = *reinterpret_cast<const uint4*>(sQ + t * TA_ROW + part * 8);
+          *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(out) +
+                                    (((static_cast<long>(b) * T + t) * HW + pos) * ld_out + head * 64 + part * 8) * 2) = v;
+        }
+      }
+    }
+    __syncthreads();                            // this buffer is free for the prefetch of the round after next
+  }
+  cp_async_wait<0>();
+}
+
 }  // namespace aab
 
 using namespace aab;
@@ -845,13 +1025,32 @@ extern "C" int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k
                                      long ld_out, int b, int t, int hw, int heads, float scale, int is_bf16,
                                      void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!qkv || !out || t < 1 || t > 32 || b < 1 || hw < 1 || heads < 1 || (ld % 8) || (ld_out % 8)) return AAB_ERR_ARG;
+  if (is_bf16 & ~3) return AAB_ERR_ARG;   // bit 0: bf16, bit 1: long-clip kernel (t <= 128)
+  const bool long_clip = (is_bf16 & 2) != 0;
+  is_bf16 &= 1;
+  if (!qkv || !out || t < 1 || t > (long_clip ? 128 : 32) || b < 1 || hw < 1 || heads < 1 || (ld % 8) || (ld_out % 8))
+    return AAB_ERR_ARG;
   if ((reinterpret_cast<uintptr_t>(qkv) % 16) || (reinterpret_cast<uintptr_t>(out) % 16) || ((q_col0 | k_col0 | v_col0) % 8))
     return AAB_ERR_ARG;                   // 16-byte pieces (cp.async gather, row stores)
   if (q_col0 < 0 || k_col0 < 0 || v_col0 < 0 || q_col0 + 64L * heads > ld || k_col0 + 64L * heads > ld ||
       v_col0 + 64L * heads > ld || 64L * heads > ld_out)
     return AAB_ERR_ARG;                   // every head's 64 columns inside a row of qkv / out
   const long total = static_cast<long>(b) * hw * heads;
+  if (long_clip) {
+    // one item per CTA at a time; TP = 64 fits four 54 KiB CTAs per SM, TP = 128 two 108 KiB CTAs
+    const int tp = t <= 64 ? 64 : 128;
+    const int smem = tp == 64 ? tal_smem_bytes<64>() : tal_smem_bytes<128>();
+    const long cap = (tp == 64 ? 4L : 2L) * num_sms();
+    const int grid = static_cast<int>(total < cap ? total : cap);
+    static std::atomic<unsigned long long> a64f{0}, a64t{0}, a128f{0}, a128t{0};
+    std::atomic<unsigned long long>& attr = tp == 64 ? (is_bf16 ? a64t : a64f) : (is_bf16 ? a128t : a128f);
+    auto kern = tp == 64 ? (is_bf16 ? temporal_attn_d64_long_kernel<true, 64> : temporal_attn_d64_long_kernel<false, 64>)
+                         : (is_bf16 ? temporal_attn_d64_long_kernel<true, 128> : temporal_attn_d64_long_kernel<false, 128>);
+    if (int r = ensure_dyn_smem(kern, smem, attr)) return r;
+    launch_k(kern, dim3(grid), dim3(TAL_THREADS), smem, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw, heads,
+             scale);
+    return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
+  }
   static int use_v1 = -1;                 // AAB_TATTN_V1=1: the round-1 kernel (A/B measurements)
   if (use_v1 < 0) {
     const char* e = getenv("AAB_TATTN_V1");

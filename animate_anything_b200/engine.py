@@ -273,7 +273,7 @@ def temporal_transformer_forward(ctx: Ctx, m: L.TransformerTemporalModel, x: tor
                 continue
             nrm = ops.layernorm(hs, bp[nk][0], bp[nk][1])
             qkv = ops.linear(nrm, bp[qk])
-            a = ops.temporal_attn_d64(qkv, g.b, g.t, g.hw, m.heads, 0, inner, 2 * inner)
+            a = ops.temporal_attn(qkv, g.b, g.t, g.hw, m.heads, 0, inner, 2 * inner)
             hs = ops.linear(a, bp[ok][0], bp[ok][1], residual=hs)
         n3 = ops.layernorm(hs, bp["n3"][0], bp["n3"][1])
         hs = _ff(ctx, bp, hs, n3)

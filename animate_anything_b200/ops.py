@@ -410,6 +410,33 @@ def temporal_attn_d64(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_
     return out
 
 
+# The long-clip kernel keeps a 16-query tile's whole score row (up to 128 keys) in registers; longer clips would need an
+# online softmax over key blocks.
+TEMPORAL_MAX_FRAMES = 128
+
+
+def temporal_attn_long(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
+    """`temporal_attn_d64` on the long-clip kernel (bit 1 of `is_bf16`): t in 1..TEMPORAL_MAX_FRAMES, same layout."""
+    bf = _is_bf16(qkv) | 2
+    out = torch.empty((qkv.shape[0], heads * 64), device=qkv.device, dtype=qkv.dtype)
+    rows = qkv.shape[0]
+    _profiled("temporal_attn_d64", 2.0 * rows * heads * 64 * 4, 4.0 * b * hw * heads * t * t * 64,
+              lambda: _lib.call("aab_temporal_attn_d64", _ptr(qkv), qkv.stride(0), q_col0, k_col0, v_col0, _ptr(out),
+                                out.stride(0), b, t, hw, heads, 1.0 / math.sqrt(64.0), bf, _stream()),
+              shape=(b, t, hw, heads))
+    return out
+
+
+def temporal_attn(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
+    """Self-attention over the t frames of every (b, pixel, head), kernel chosen by t: up to 32 frames the v2 kernel
+    (`temporal_attn_d64`, unchanged results), 33..TEMPORAL_MAX_FRAMES the long-clip kernel."""
+    if t <= 32:
+        return temporal_attn_d64(qkv, b, t, hw, heads, q_col0, k_col0, v_col0)
+    if t <= TEMPORAL_MAX_FRAMES:
+        return temporal_attn_long(qkv, b, t, hw, heads, q_col0, k_col0, v_col0)
+    raise NotImplementedError(f"temporal attention handles up to {TEMPORAL_MAX_FRAMES} frames, got {t}")
+
+
 # ---------------------------------------------------------------------------------------------- norms
 _gn_ws = {}
 

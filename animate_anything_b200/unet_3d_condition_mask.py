@@ -260,6 +260,9 @@ class UNet3DConditionModel(ModelBase):
         if down_block_additional_residuals is not None or mid_block_additional_residual is not None:
             raise NotImplementedError("ControlNet residuals (:456-479) are not used by any caller in the reference tree and "
                                       "are not implemented")
+        if sample.shape[2] + 1 > ops.TEMPORAL_MAX_FRAMES:   # F + 1 frames (condition frame); raise before the first launch
+            raise NotImplementedError(f"temporal attention handles up to {ops.TEMPORAL_MAX_FRAMES} frames: {sample.shape[2]} "
+                                      f"frames + the condition frame is {sample.shape[2] + 1}")
         prep = self._prepared()
         own = prep.get(self)
         dt = prep.dtype

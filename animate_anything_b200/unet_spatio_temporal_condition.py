@@ -16,7 +16,7 @@ Same constructor config, sub-module names (-> state_dict keys) and forward signa
                                 every pixel with the gather-in-kernel temporal attention, no permutes) + AlphaBlender
 Activation layout as in engine.py: [rows, C] with rows = (b, f, y, x).
 
-Restrictions (raise, never fall back): attention head dim 64 (the SVD checkpoints: 320/5, 640/10, 1280/20), F <= 32, 16-bit
+Restrictions (raise, never fall back): attention head dim 64 (the SVD checkpoints: 320/5, 640/10, 1280/20), F <= 128, 16-bit
 weights on a CUDA device.  Parity: tests/test_gpu_svd.py against the oracle restatement (oracle/shim/diffusers/_svd.py —
 leaf semantics recalled from diffusers 0.24, unpinned; composition pinned to the verbatim reference pipeline).
 """
@@ -193,8 +193,6 @@ def st_resblock_forward(ctx: E.Ctx, m: SpatioTemporalResBlock, x, g: E.Geo, skip
 def st_transformer_forward(ctx: E.Ctx, m: TransformerSpatioTemporalModel, x, g: E.Geo):
     p = ctx.prep.get(m)
     inner = m.heads * 64
-    if g.t > 32:
-        raise NotImplementedError("temporal attention kernel handles up to 32 frames (SVD: 14 / 25)")
     hs = ops.groupnorm(x, g.n, g.hw, p["n"][0], p["n"][1], 1e-6, False, 32)
     hs = ops.linear(hs, p["pi"][0], p["pi"][1])
     # frame position embedding: time_pos_embed(time_proj(arange(F)))  -> fp32 [F, C]
@@ -220,7 +218,7 @@ def st_transformer_forward(ctx: E.Ctx, m: TransformerSpatioTemporalModel, x, g: 
         h = ops.linear(f, tp["ffi2"][0], tp["ffi2"][1], residual=mix)
         n = ops.layernorm(h, tp["n1"][0], tp["n1"][1])
         qkv = ops.linear(n, tp["qkv1"])
-        a = ops.temporal_attn_d64(qkv, g.b, g.t, g.hw, m.heads, 0, inner, 2 * inner)
+        a = ops.temporal_attn(qkv, g.b, g.t, g.hw, m.heads, 0, inner, 2 * inner)
         h = ops.linear(a, tp["o1"][0], tp["o1"][1], residual=h)
         if tblk.attn2 is not None:
             # diffusers builds `time_context` in (h*w, batch) order but the block's tokens are (batch, h*w): token (b, s)
@@ -513,9 +511,6 @@ class UNetSpatioTemporalConditionModel(ModelBase):
                 return_dict: bool = True, _raw: bool = False, _x16: Optional[torch.Tensor] = None, _shape=None):
         """`_x16` / `_shape` (used by the fused SVD loop, pipeline_svd.py): the channels-last, 16-channel-padded input
         [B*F, h, w, 16] already assembled by `aab_svd_in_assemble`, with `_shape` = (B, F, C, h, w); `sample` is ignored."""
-        prep = self._prepared()
-        own = prep.get(self)
-        dt, dev = prep.dtype, prep.device
         cfg = self.config
         if _x16 is not None:
             b, nf, c, h, w = _shape
@@ -523,6 +518,11 @@ class UNetSpatioTemporalConditionModel(ModelBase):
             if sample.dim() != 5 or sample.shape[2] != cfg.in_channels:
                 raise ValueError(f"sample must be [batch, frames, {cfg.in_channels}, height, width], got {tuple(sample.shape)}")
             b, nf, c, h, w = sample.shape
+        if nf > ops.TEMPORAL_MAX_FRAMES:       # before the first launch, not halfway through the forward
+            raise NotImplementedError(f"temporal attention handles up to {ops.TEMPORAL_MAX_FRAMES} frames, got {nf}")
+        prep = self._prepared()
+        own = prep.get(self)
+        dt, dev = prep.dtype, prep.device
         if any(s % (2 ** self.num_upsamplers) for s in (h, w)):
             raise ValueError("latent height/width must be multiples of 2**num_upsamplers (diffusers' SVD UNet has no "
                              "upsample_size path either)")

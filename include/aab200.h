@@ -68,10 +68,12 @@ int aab_clip_image_prep(const void* src, int src_type, long sb, long sc, long sy
                         const float* taps_y, int ks_y, const float* taps_x, int ks_x, const float* mean_std, int out_size,
                         int patch, void* out, long ld_out, int is_bf16, void* stream);
 
-/* Self-attention over the frame axis (T <= 32) without the (b t) c h w -> (b h w) t c permutes
+/* Self-attention over the frame axis without the (b t) c h w -> (b h w) t c permutes
  * (diffusers TransformerTemporalModel.forward; models/unet_3d_blocks.py:299-306,459-467,694-701).
- * qkv rows ((b t) hw, ld); head h of q / k / v at columns col0 + 64 h.  Rejected with 1: t outside 1..32, b, hw or heads < 1,
- * col0 + 64 heads > ld, 64 heads > ld_out, ld / ld_out / col0 not multiples of 8, qkv / out not 16-byte aligned. */
+ * qkv rows ((b t) hw, ld); head h of q / k / v at columns col0 + 64 h.  is_bf16 bit 0: bf16 (else fp16); bit 1: the long-clip
+ * kernel, t in 1..128 (without it t in 1..32, the v2 kernel).  Rejected with 1: any other is_bf16 bit, t outside the
+ * selected range, b, hw or heads < 1, col0 + 64 heads > ld, 64 heads > ld_out, ld / ld_out / col0 not multiples of 8,
+ * qkv / out not 16-byte aligned. */
 int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k_col0, int v_col0, void* out, long ld_out, int b, int t,
                           int hw, int heads, float scale, int is_bf16, void* stream);
 
