@@ -125,6 +125,16 @@ class AutoencoderKLTemporalDecoder(AutoencoderKL):
     def decode_chunk_video(self, z: torch.Tensor, num_frames: int) -> torch.Tensor:
         """z [batch*num_frames, 4, h, w] -> fp32 video [batch, 3, num_frames, 8h, 8w] holding the 16-bit-rounded values
         (what `decode(...).sample.float()` gives after the pipeline's reshape/permute, models/pipeline.py:456)."""
+        return self._decode_temporal(z, num_frames, u8=False)
+
+    @torch.no_grad()
+    def decode_chunk_frames_u8(self, z: torch.Tensor, num_frames: int) -> torch.Tensor:
+        """z [batch*num_frames, 4, h, w] -> uint8 frames [num_frames, 8h, batch*8w, 3]: the values of `decode_chunk_video`
+        through the SVD pipelines' `postprocess(..., "pil")` ((x / 2 + 0.5).clamp(0, 1) * 255, rounded half to even),
+        computed in the decoder's last kernel so that only uint8 frames leave the device."""
+        return self._decode_temporal(z, num_frames, u8=True)
+
+    def _decode_temporal(self, z, num_frames, u8):
         prep = self._prepared()
         own = prep.get(self)
         n, _, hh, ww = z.shape
@@ -149,7 +159,10 @@ class AutoencoderKLTemporalDecoder(AutoencoderKL):
         h = ops.groupnorm(h, g.n, g.hw, own["dec_norm"][0], own["dec_norm"][1], 1e-6, True, 32)
         y8 = ops.conv3x3(h.view(g.n, g.h, g.w, c0), own["dec_out"][0], own["dec_out"][1])          # [rows, 8] 16-bit
         y = ops.tconv3(y8, g.b, g.t, g.hw, own["dec_time"][0], own["dec_time"][1], out_f32=True)   # frame-axis conv
-        return ops.vae_dec_finalize(y, g.b, g.t, g.h, g.w, prep.dtype == torch.bfloat16)             # [b, 3, f, H, W] fp32
+        bf16 = prep.dtype == torch.bfloat16
+        if u8:
+            return ops.vae_dec_finalize_u8(y, g.b, g.t, g.h, g.w, bf16, round_half_even=True)      # [f, H, b*W, 3] uint8
+        return ops.vae_dec_finalize(y, g.b, g.t, g.h, g.w, bf16)                                   # [b, 3, f, H, W] fp32
 
     def decode_video(self, *a, **k):
         raise NotImplementedError("use decode(z, num_frames) (diffusers AutoencoderKLTemporalDecoder surface)")

@@ -621,7 +621,10 @@ __global__ void vae_dec_finalize_kernel(const float* __restrict__ y, int ldc, fl
 // decoder tail fused with diffusers tensor2vid (models/pipeline.py:205): conv_out result [B*F, H, W, ldc] (fp32) ->
 // uint8 frames [F, H, B*W, 3]:  x -> round to model dtype -> x*0.5 -> +0.5 -> clamp(0,1) -> *255 -> truncate
 // (separate fp32 multiply and add, like `video.mul_(std).add_(mean)`; numpy `astype("uint8")` truncates).
-template <bool BF16>
+// RINT: the SVD pipelines' `postprocess(..., "pil")` instead -- `(x / 2 + 0.5).clamp(0, 1)` in fp32, then numpy's
+// `(images * 255).round().astype("uint8")`: the fp32 product rounded half to even.  x / 2 and x * 0.5 are the same exact
+// value, so the steps before the last one are shared.
+template <bool BF16, bool RINT>
 __global__ void vae_dec_finalize_u8_kernel(const float* __restrict__ y, int ldc, uint8_t* __restrict__ out, int B, int F,
                                            int H, int W) {
   pdl_trigger();
@@ -642,7 +645,8 @@ __global__ void vae_dec_finalize_u8_kernel(const float* __restrict__ y, int ldc,
     v = BF16 ? __bfloat162float(__float2bfloat16_rn(v)) : __half2float(__float2half_rn(v));
     v = __fadd_rn(__fmul_rn(v, 0.5f), 0.5f);
     v = fminf(fmaxf(v, 0.0f), 1.0f);
-    out[i * 3 + c] = static_cast<uint8_t>(__fmul_rn(v, 255.0f));
+    const float s = __fmul_rn(v, 255.0f);
+    out[i * 3 + c] = static_cast<uint8_t>(RINT ? rintf(s) : s);
   }
 }
 
@@ -1014,12 +1018,18 @@ extern "C" int aab_vae_dec_finalize(const float* y, int ldc, float* out, int b, 
 
 extern "C" int aab_vae_dec_finalize_u8(const float* y, int ldc, void* out, int b, int f, int h, int w, int is_bf16,
                                        void* stream_) {
+  // bit 0: bf16 model; bit 1: round to nearest even (SVD postprocess) instead of truncating (tensor2vid)
+  if (is_bf16 & ~3) return AAB_ERR_ARG;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const long total = static_cast<long>(b) * f * h * w;
-  if (is_bf16)
-    launch_k(vae_dec_finalize_u8_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, reinterpret_cast<uint8_t*>(out), b, f, h, w);
-  else
-    launch_k(vae_dec_finalize_u8_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, reinterpret_cast<uint8_t*>(out), b, f, h, w);
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  const dim3 grid(AAB_GRID(total, 256)), block(256);
+  switch (is_bf16) {
+    case 0: launch_k(vae_dec_finalize_u8_kernel<false, false>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
+    case 1: launch_k(vae_dec_finalize_u8_kernel<true, false>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
+    case 2: launch_k(vae_dec_finalize_u8_kernel<false, true>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
+    default: launch_k(vae_dec_finalize_u8_kernel<true, true>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
+  }
   AAB_LAUNCH_RET();
 }
 

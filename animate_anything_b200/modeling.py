@@ -95,18 +95,34 @@ class ModelBase(nn.Module):
         return cls(**kw)
 
     @classmethod
+    def _weight_files(cls, variant=None):
+        """(safetensors name, pickle name) of the checkpoint; a `variant` goes before the extension, as diffusers and
+        transformers name it (`diffusion_pytorch_model.fp16.safetensors`, `pytorch_model.fp16.bin`)."""
+        names = (cls.weights_name + ".safetensors", cls.weights_bin_name or (cls.weights_name + ".bin"))
+        if variant is None:
+            return names
+        return tuple(f"{stem}.{variant}{ext}" for stem, ext in (os.path.splitext(n) for n in names))
+
+    @classmethod
     def from_pretrained(cls, path, subfolder=None, torch_dtype=None, ignore_mismatched_sizes=False,
-                        low_cpu_mem_usage=False, device_map=None, **overrides):
+                        low_cpu_mem_usage=False, device_map=None, variant=None, **overrides):
         root = os.path.join(path, subfolder) if subfolder else path
         with open(os.path.join(root, cls.config_name)) as f:
             cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
+        st_name, bin_name = cls._weight_files(variant)
+        if variant is not None and not any(os.path.exists(os.path.join(root, n)) for n in (st_name, bin_name)):
+            plain = cls._weight_files()
+            found = [n for n in plain if os.path.exists(os.path.join(root, n))]
+            raise FileNotFoundError(f"no {st_name} or {bin_name} in {root} (variant={variant!r})"
+                                    + (f"; {found[0]} exists: load it without `variant`" if found else
+                                       f", and no {plain[0]} or {plain[1]} either"))
         model = cls.from_config(cfg, **overrides)
-        st_path = os.path.join(root, cls.weights_name + ".safetensors")
+        st_path = os.path.join(root, st_name)
         if os.path.exists(st_path):
             from safetensors.torch import load_file
             sd = load_file(st_path)
         else:
-            sd = torch.load(os.path.join(root, cls.weights_bin_name or (cls.weights_name + ".bin")), map_location="cpu")
+            sd = torch.load(os.path.join(root, bin_name), map_location="cpu")
         if ignore_mismatched_sizes:
             own = model.state_dict()
             sd = {k: v for k, v in sd.items() if k in own and own[k].shape == v.shape}

@@ -719,10 +719,13 @@ def vae_dec_finalize(y: torch.Tensor, b, f, h, w, bf16: bool) -> torch.Tensor:
     return out
 
 
-def vae_dec_finalize_u8(y: torch.Tensor, b, f, h, w, bf16: bool) -> torch.Tensor:
-    """conv_out result -> uint8 frames [f, h, b*w, 3] (diffusers tensor2vid layout and rounding)."""
+def vae_dec_finalize_u8(y: torch.Tensor, b, f, h, w, bf16: bool, round_half_even: bool = False) -> torch.Tensor:
+    """conv_out result -> uint8 frames [f, h, b*w, 3] (diffusers tensor2vid layout and rounding: the scaled value is
+    truncated).  `round_half_even`: the SVD pipelines' `postprocess(..., "pil")` rounding instead, numpy's
+    `((x / 2 + 0.5).clamp(0, 1) * 255).round()` on the fp32 product (bit 1 of the entry point's flag)."""
     out = torch.empty((f, h, b * w, 3), device=y.device, dtype=torch.uint8)
-    _lib.call("aab_vae_dec_finalize_u8", _ptr(y), y.stride(0), _ptr(out), b, f, h, w, int(bf16), _stream())
+    _lib.call("aab_vae_dec_finalize_u8", _ptr(y), y.stride(0), _ptr(out), b, f, h, w,
+              int(bf16) | (2 if round_half_even else 0), _stream())
     return out
 
 

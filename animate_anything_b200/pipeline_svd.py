@@ -1,5 +1,7 @@
-"""Mirror of the reference's `MaskStableVideoDiffusionPipeline.__call__` (models/pipeline.py:223-466; BASELINE config
-4, driven by train_svd.py:756-777): same keyword arguments, defaults and return values.
+"""Mirror of diffusers 0.24 `StableVideoDiffusionPipeline` (loading, the stock image-to-video `__call__`) and of the
+reference's `MaskStableVideoDiffusionPipeline.__call__` (models/pipeline.py:223-466; BASELINE config 4, driven by
+train_svd.py:756-777) and `TextStableVideoDiffusionPipeline.__call__` (:468-731): same keyword arguments, defaults and
+return values.  `output_type="pil"` frames are rounded to uint8 in the decoder's last kernel (`decode_chunk_frames_u8`).
 
 What is mirrored on the sm_90a kernels (the hot path, reference line -> here):
   :359-362  `_encode_vae_image` (VAE encode of the noise-augmented image, `latent_dist.mode()`)  -> AutoencoderKLTemporalDecoder.encode
@@ -36,7 +38,14 @@ def _append_dims(x, target_dims):
     return x[(...,) + (None,) * dims_to_append]
 
 
-class MaskStableVideoDiffusionPipeline:
+class StableVideoDiffusionPipeline:
+    """Mirror of diffusers 0.24 `StableVideoDiffusionPipeline`, the object both SVD entry points build
+    (`StableVideoDiffusionPipeline.from_pretrained(path, torch_dtype=torch.float16, variant="fp16")`, train_svd.py:87 and
+    app_svd.py:37), and the base of the Mask / Text pipelines as in the reference (models/pipeline.py:223,468).  Everything
+    their `__call__`s touch lives here, because the reference calls them unbound on a stock instance
+    (`MaskStableVideoDiffusionPipeline.__call__(pipeline, ...)`, train_svd.py:766; `TextStableVideoDiffusionPipeline.__call__(
+    self.pipeline, ...)`, app_svd.py:120)."""
+
     def __init__(self, vae, image_encoder, unet, scheduler, feature_extractor=None):
         self.vae, self.image_encoder, self.unet, self.scheduler = vae, image_encoder, unet, scheduler
         self.feature_extractor = feature_extractor
@@ -44,6 +53,56 @@ class MaskStableVideoDiffusionPipeline:
         from .image_processor import VaeImageProcessor
         self.image_processor = VaeImageProcessor(vae_scale_factor=self.vae_scale_factor)
         self.last_gpu_launches = 0
+
+    @classmethod
+    def from_pretrained(cls, path, torch_dtype=None, variant=None, unet=None, vae=None, image_encoder=None, scheduler=None,
+                        feature_extractor=None):
+        """Reads the diffusers SVD checkpoint layout: `unet/`, `vae/` (diffusers weight names), `image_encoder/`
+        (transformers names, `model.safetensors`), `scheduler/scheduler_config.json` and
+        `feature_extractor/preprocessor_config.json` (its `image_mean` / `image_std` are what the CLIP preprocessing
+        reads).  `variant="fp16"` loads `*.fp16.safetensors` / `*.fp16.bin` weights.  A component passed as a keyword is
+        used as it is instead of being loaded; a missing `image_encoder/` or `feature_extractor/` folder leaves None."""
+        import json
+        import os
+        from .autoencoder_kl_temporal_decoder import AutoencoderKLTemporalDecoder
+        from .clip_vision import CLIPVisionModelWithProjection
+        from .modeling import FrozenConfig
+        from .schedulers import EulerDiscreteScheduler
+        from .unet_spatio_temporal_condition import UNetSpatioTemporalConditionModel
+        kw = dict(torch_dtype=torch_dtype, variant=variant)
+        if unet is None:
+            unet = UNetSpatioTemporalConditionModel.from_pretrained(path, subfolder="unet", **kw)
+        if vae is None:
+            vae = AutoencoderKLTemporalDecoder.from_pretrained(path, subfolder="vae", **kw)
+        if image_encoder is None and os.path.isdir(os.path.join(path, "image_encoder")):
+            image_encoder = CLIPVisionModelWithProjection.from_pretrained(path, subfolder="image_encoder", **kw)
+        if scheduler is None:
+            scheduler = EulerDiscreteScheduler.from_pretrained(path, subfolder="scheduler")
+        fe_path = os.path.join(path, "feature_extractor", "preprocessor_config.json")
+        if feature_extractor is None and os.path.exists(fe_path):
+            with open(fe_path) as f:
+                feature_extractor = FrozenConfig(json.load(f))
+        return cls(vae=vae, image_encoder=image_encoder, unet=unet, scheduler=scheduler, feature_extractor=feature_extractor)
+
+    def to(self, *args, device=None, dtype=None):
+        """`pipeline.to("cuda")` / `.to(torch.float16)` / `.to(device=..., dtype=...)`: moves the UNet, VAE and image encoder."""
+        for a in args:
+            if isinstance(a, torch.dtype):
+                dtype = a
+            else:
+                device = a
+        for m in (self.vae, self.unet, self.image_encoder):
+            if isinstance(m, torch.nn.Module):
+                m.to(device=device, dtype=dtype)
+        return self
+
+    @property
+    def device(self):
+        return self.unet.device
+
+    @property
+    def dtype(self):
+        return self.unet.dtype
 
     @property
     def guidance_scale(self):
@@ -135,6 +194,109 @@ class MaskStableVideoDiffusionPipeline:
             outs.append(self.vae.decode_chunk_video(z, z.shape[0]))           # [1, 3, n, H, W] fp32
         return torch.cat(outs, dim=2)                                         # [1, 3, F, H, W]: chunks are consecutive frames
 
+    def _output_frames(self, latents, num_frames, decode_chunk_size, output_type):
+        """diffusers svd_tensor2vid(decode_latents(...), image_processor, output_type) -> one list / array / tensor of
+        frames per video.  "pil" decodes each chunk straight to uint8 frames on the device (the decoder's last kernel
+        rounds like `postprocess`), so one uint8 copy per chunk is all that reaches the host; the other types keep the
+        fp32 video and `image_processor.postprocess`."""
+        if output_type == "latent":
+            return latents
+        if output_type != "pil":
+            frames = self.decode_latents(latents, num_frames, decode_chunk_size)
+            return [self.image_processor.postprocess(frames[b].permute(1, 0, 2, 3), output_type)
+                    for b in range(frames.shape[0])]                          # diffusers svd tensor2vid
+        import PIL.Image
+        if latents.shape[0] != 1:
+            raise NotImplementedError("one video per call (as the reference's mask handling implies, models/pipeline.py:372)")
+        lat = latents.flatten(0, 1)
+        inv = 1.0 / self.vae.config.scaling_factor
+        images = []
+        for i in range(0, lat.shape[0], decode_chunk_size):
+            z = (lat[i: i + decode_chunk_size] * inv).contiguous()          # as decode_latents
+            u8 = self.vae.decode_chunk_frames_u8(z, z.shape[0]).cpu().numpy()   # [n, H, W, 3]
+            images.extend(PIL.Image.fromarray(im) for im in u8)
+        return [images]
+
+    @torch.no_grad()
+    def __call__(self, image, height: int = 576, width: int = 1024, num_frames: Optional[int] = None,
+                 num_inference_steps: int = 25, min_guidance_scale: float = 1.0, max_guidance_scale: float = 3.0,
+                 fps: int = 7, motion_bucket_id: int = 127, noise_aug_strength: float = 0.02,
+                 decode_chunk_size: Optional[int] = None, num_videos_per_prompt: Optional[int] = 1,
+                 generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None,
+                 latents: Optional[torch.Tensor] = None, output_type: Optional[str] = "pil",
+                 callback_on_step_end: Optional[Callable[[int, int, Dict], None]] = None,
+                 callback_on_step_end_tensor_inputs: List[str] = ["latents"], return_dict: bool = True,
+                 image_embeddings: Optional[torch.Tensor] = None):
+        """diffusers 0.24 `StableVideoDiffusionPipeline.__call__` (image-to-video with an 8-channel UNet): the loop of the
+        Mask call without the mask, i.e. `cat([latent_model_input, image_latents], dim=2)` with zeroed image latents in the
+        unconditional half.  The input assembly, UNet, per-frame CFG + Euler step and temporal decode run on the sm_90a
+        kernels.  One video per call.  Deviation: the stock call encodes the image with an fp32 VAE when
+        `vae.config.force_upcast` (`needs_upcasting`); the sm_90a path is 16-bit, so the encode runs in the model dtype."""
+        from . import _lib
+        in_ch = self.unet.config.in_channels
+        if in_ch != 8:
+            raise ValueError(f"StableVideoDiffusionPipeline needs an 8-channel UNet (cat([latents, image_latents])), this one "
+                             f"has in_channels={in_ch}; 9-channel motion-mask UNets go through "
+                             "MaskStableVideoDiffusionPipeline / TextStableVideoDiffusionPipeline")
+        launches0 = _lib.launch_count()
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        num_frames = num_frames if num_frames is not None else self.unet.config.num_frames
+        decode_chunk_size = decode_chunk_size if decode_chunk_size is not None else num_frames
+        self.check_inputs(image, height, width)
+        device, dtype = self.unet.device, self.unet.dtype
+        cfg = max_guidance_scale > 1.0
+        image_t = self.image_processor.preprocess(image, height=height, width=width).to(device)
+        batch_size = image_t.shape[0]
+        if batch_size * num_videos_per_prompt != 1:
+            raise NotImplementedError("one video per call on the sm_90a path")
+        if image_embeddings is None:
+            image_embeddings = self._encode_image(image_t, device, num_videos_per_prompt, cfg, raw_image=image)
+        else:
+            image_embeddings = image_embeddings.to(device=device, dtype=dtype)
+            if cfg and image_embeddings.shape[0] == batch_size:
+                image_embeddings = torch.cat([torch.zeros_like(image_embeddings), image_embeddings])
+        fps = fps - 1
+        noise = torch.randn(image_t.shape, generator=generator, device=generator.device if generator is not None else device,
+                            dtype=image_t.dtype).to(device)
+        image_t = image_t + noise_aug_strength * noise
+        lat_h, lat_w = height // self.vae_scale_factor, width // self.vae_scale_factor
+        il = self.vae.encode(image_t.to(dtype)).latent_dist.mode().to(dtype).contiguous()              # [1, 4, h, w]
+        cond = il.reshape(1, batch_size, 1, 4, lat_h, lat_w)
+        ids = torch.tensor([[fps, motion_bucket_id, noise_aug_strength]], dtype=dtype).repeat(batch_size, 1)
+        ids = (torch.cat([ids, ids]) if cfg else ids).to(device)
+        self.scheduler.set_timesteps(num_inference_steps, device=device)
+        timesteps = self.scheduler.timesteps
+        sigmas = [float(s) for s in self.scheduler.sigmas]
+        shape = (batch_size, num_frames, in_ch // 2, lat_h, lat_w)
+        if latents is None:
+            latents = torch.randn(shape, generator=generator, device=generator.device if generator is not None else device,
+                                  dtype=dtype).to(device)
+        else:
+            latents = latents.to(device=device, dtype=dtype)
+        latents = (latents * float(self.scheduler.init_noise_sigma)).contiguous()
+        gs = torch.linspace(min_guidance_scale, max_guidance_scale, num_frames).unsqueeze(0).to(device, latents.dtype)
+        self._guidance_scale = _append_dims(gs.repeat(batch_size, 1), latents.ndim)
+        gs_f32 = gs[0].float().contiguous()
+        b_unet = (2 if cfg else 1) * batch_size
+        self._num_timesteps = len(timesteps)
+        for i, t in enumerate(timesteps):
+            x16 = ops.svd_in_assemble_frames(latents, cond, None, sigmas[i], cfg, True)
+            pred, _ = self.unet(None, t, image_embeddings, ids, _raw=True, _x16=x16,
+                                _shape=(b_unet, num_frames, in_ch, lat_h, lat_w))
+            latents = ops.svd_cfg_euler_step(pred, cfg, gs_f32, latents, sigmas[i], sigmas[i + 1])
+            if callback_on_step_end is not None:
+                callback_kwargs = {k: locals()[k] for k in callback_on_step_end_tensor_inputs}
+                callback_outputs = callback_on_step_end(self, i, t, callback_kwargs)
+                latents = callback_outputs.pop("latents", latents)
+        frames = self._output_frames(latents, num_frames, decode_chunk_size, output_type)
+        self.last_gpu_launches = _lib.launch_count() - launches0
+        if not return_dict:
+            return frames
+        return StableVideoDiffusionPipelineOutput(frames=frames)
+
+
+class MaskStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
     @torch.no_grad()
     def __call__(self, image, height: int = 576, width: int = 1024, num_frames: Optional[int] = None,
                  num_inference_steps: int = 25, min_guidance_scale: float = 1.0, max_guidance_scale: float = 3.0,
@@ -208,19 +370,14 @@ class MaskStableVideoDiffusionPipeline:
                 callback_kwargs = {k: locals()[k] for k in callback_on_step_end_tensor_inputs}
                 callback_outputs = callback_on_step_end(self, i, t, callback_kwargs)
                 latents = callback_outputs.pop("latents", latents)
-        if output_type != "latent":
-            frames = self.decode_latents(latents, num_frames, decode_chunk_size)
-            frames = [self.image_processor.postprocess(frames[b].permute(1, 0, 2, 3), output_type)
-                      for b in range(frames.shape[0])]                       # diffusers svd tensor2vid
-        else:
-            frames = latents
+        frames = self._output_frames(latents, num_frames, decode_chunk_size, output_type)
         self.last_gpu_launches = _lib.launch_count() - launches0
         if not return_dict:
             return frames
         return StableVideoDiffusionPipelineOutput(frames=frames)
 
 
-class TextStableVideoDiffusionPipeline(MaskStableVideoDiffusionPipeline):
+class TextStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
     """Mirror of the reference's `TextStableVideoDiffusionPipeline.__call__` (models/pipeline.py:468-731): the SVD loop
     conditioned on the CLIP image embedding (`condition_type="image"`), on text embeddings (`"text"`: prompt_embeds [B, 77, D]
     replace the image embedding, :579-582) or on both (any other value: image token + text tokens concatenated, 78 keys, :583-587);
@@ -323,12 +480,7 @@ class TextStableVideoDiffusionPipeline(MaskStableVideoDiffusionPipeline):
                 callback_kwargs = {k: locals()[k] for k in callback_on_step_end_tensor_inputs}
                 callback_outputs = callback_on_step_end(self, i, t, callback_kwargs)
                 latents = callback_outputs.pop("latents", latents)
-        if output_type != "latent":
-            frames = self.decode_latents(latents, num_frames, decode_chunk_size)
-            frames = [self.image_processor.postprocess(frames[b].permute(1, 0, 2, 3), output_type)
-                      for b in range(frames.shape[0])]
-        else:
-            frames = latents
+        frames = self._output_frames(latents, num_frames, decode_chunk_size, output_type)
         self.last_gpu_launches = _lib.launch_count() - launches0
         if not return_dict:
             return frames

@@ -168,7 +168,9 @@ int aab_vae_enc_finalize(const void* mom, int ldm, const float* wq, const float*
 int aab_vae_dec_in(const void* lat, float inv_scale, const float* wp, const float* bp, void* out, int b, int f, int h, int w,
                    int is_bf16, void* stream);
 int aab_vae_dec_finalize(const float* y, int ldc, float* out, int b, int f, int h, int w, int is_bf16, void* stream);
-/* decoder tail fused with diffusers tensor2vid (models/pipeline.py:205): uint8 frames [f, h, b*w, 3] */
+/* decoder tail fused with diffusers tensor2vid (models/pipeline.py:205): uint8 frames [f, h, b*w, 3].  is_bf16 bit 0: bf16
+ * model; bit 1: round the scaled value half to even (the SVD pipelines' postprocess) instead of truncating; any other bit
+ * returns 1 before a launch. */
 int aab_vae_dec_finalize_u8(const float* y, int ldc, void* out, int b, int f, int h, int w, int is_bf16, void* stream);
 
 /* Forward-diffuse the image latent to the first kept timestep: out = sa * repeat(x0 over f) + sb * noise with torch's
