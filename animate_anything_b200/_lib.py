@@ -15,6 +15,7 @@ MAX_TAPS = 9
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_QUICK_GELU = 0, 1, 2, 3
 F_BF16, F_DIRECT, F_OUT_F32, F_GEGLU, F_SCALE_ACC, F_PAIR = 1, 2, 4, 8, 16, 32
 F_QUAD = 16384
+F_TWO_CTA = 64
 
 
 class IgemmDesc(C.Structure):

@@ -13,6 +13,10 @@
 // * Persistent CTAs (one per SM) walk the tile list n-fastest so that the CTAs running concurrently share the same
 //   A rows (L2 hits) while the weights stay L2-resident; the producer runs ahead into the next tile while the
 //   consumers finish the epilogue of the current one.
+// * Two CTAs per SM (AAB_F_TWO_CTA, template MINB = 2, 64-column tiles, 3-stage ring, 80 registers per thread) for the
+//   1-tap launches with K <= 640 (ops.pick_two_cta): their main loop is only 5 - 10 k-blocks, so with one CTA the tensor
+//   cores idle through every epilogue; the second CTA's MMAs run under it.  Same control flow, K order and epilogue:
+//   bit-identical to one CTA per SM.
 // * Clusters (IgemmParams::cluster = 2 or 4, 256-column tiles): the CTAs of a cluster take consecutive m-tiles of the same
 //   n-tile; each fetches 1/cluster of the weight tile and multicasts it to all of them, so a k-block reads the weights from
 //   L2 once per cluster instead of once per CTA.  A stage is refilled only after the consumers of every CTA of the cluster
@@ -47,16 +51,29 @@ constexpr int NUM_CONSUMER_WARPS = 4 * NUM_CONSUMERS;
 constexpr int SLAB_COLS = 32;
 constexpr int SLAB_BYTES = 16 * SLAB_COLS * 2;   // 1 KiB
 
-// smem ring depth per tile width: 160 - 200 KiB of operands in flight whatever BN, plus the column-statistics scratch and the
-// epilogue slabs, inside the 227 KiB a block may use
-template <int BN>
+// Shared-memory ring and register split per tile width and CTAs per SM (MINB).
+//   MINB = 1: 160 - 200 KiB of operands in flight whatever BN, plus the column-statistics scratch and the epilogue slabs,
+//             inside the 227 KiB a block may use; the producer warpgroup gives registers to the consumers (40 / 232).
+//   MINB = 2: the short-K 1-tap launches (ops.pick_two_cta), 64-column tiles only: two CTAs per SM, so that one CTA's
+//             epilogue and ring refill run under the other's MMAs.  Shared memory: a CTA gets at most 113 KiB (half of the SM's
+//             228 KiB less the 1 KiB reserved per CTA); 3 stages = 72 KiB of operands + 4 KiB statistics + 16 KiB slabs +
+//             pad = 93.25 KiB (a fourth stage would need 117.25).  Registers: __launch_bounds__(384, 2) caps every thread at
+//             80 (2 x 384 x 80 <= 64 K), 30 720 per CTA = producer 32 + consumers 104.  The compiler allocates the consumer
+//             code within the 80 of the launch bounds: the 32 accumulators of BN = 64 fit with no spill, the 64 of
+//             BN = 128 (and so GEGLU) do not compile.  A producer below 32 spills its tile / tap coordinates.
+template <int BN, int MINB = 1>
 struct Cfg {
-  static constexpr int STAGES = (BN >= 192) ? 4 : (BN == 160) ? 5 : (BN == 128) ? 6 : 8;
+  static_assert(MINB == 1 || (MINB == 2 && BN == 64), "two CTAs per SM are instantiated at BN = 64 only");
+  static constexpr int STAGES = (MINB == 2) ? 3 : (BN >= 192) ? 4 : (BN == 160) ? 5 : (BN == 128) ? 6 : 8;
+  static constexpr int PRODUCER_REGS = (MINB == 2) ? 32 : 40;
+  static constexpr int CONSUMER_REGS = (MINB == 2) ? 104 : 232;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STATS_BYTES = NUM_CONSUMER_WARPS * BN * 2 * 4;   // per-warp (sum, sum of squares) per column
   static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + STATS_BYTES +
                                     NUM_CONSUMER_WARPS * 2 * SLAB_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  static_assert(SMEM_BYTES <= 227 * 1024, "tile configuration exceeds the shared memory of an SM");
+  static_assert(SMEM_BYTES <= (MINB == 2 ? 113 : 227) * 1024, "tile configuration exceeds the shared memory of an SM");
+  static_assert(128 * PRODUCER_REGS + 128 * NUM_CONSUMERS * CONSUMER_REGS <= NUM_THREADS * (MINB == 2 ? 80 : 168),
+                "setmaxnreg split exceeds the registers the launch bounds give a CTA");
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -83,12 +100,12 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_addr, uint32_t
 //                              bias / SiLU, no scaling; goes through the warp's shared-memory slab and leaves as 16-byte
 //                              stores of whole 64-byte row segments; may emit column statistics
 //   direct  (AAB_F_DIRECT):    any n_out, fp32 or 16-bit output, every flag combination, masked per element
-template <int BN, bool GEGLU, bool BF16>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+template <int BN, int MINB, bool GEGLU, bool BF16>
+__global__ void __launch_bounds__(NUM_THREADS, MINB)
 igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
              const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
   pdl_trigger();
-  using CF = Cfg<BN>;
+  using CF = Cfg<BN, MINB>;
   constexpr int STAGES = CF::STAGES;
   constexpr int OUT_BN = GEGLU ? BN / 2 : BN;
   extern __shared__ uint8_t smem_raw[];
@@ -131,7 +148,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 
   if (wg == 0) {
     // ===================================================== TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<CF::PRODUCER_REGS>();
     if (warp == 0 && elect_one()) {
       // the weight tile is fetched in NS row slices of BN / NS rows (GEGLU: values and gates are separate slices); CTA crank
       // of the cluster fetches slices crank, crank + CL, ... and multicasts them
@@ -186,7 +203,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   }
 
   // ===================================================== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64)
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<CF::CONSUMER_REGS>();
   const int cw = wg - 1;
   const int wq = warp & 3;
   const int lane = static_cast<int>(lane_id());
@@ -469,12 +486,12 @@ int num_sms() {
   return g_num_sms;
 }
 
-template <int BN, bool GEGLU, bool BF16>
+template <int BN, int MINB, bool GEGLU, bool BF16>
 static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
                     int max_ctas, cudaStream_t stream) {
-  using CF = Cfg<BN>;
+  using CF = Cfg<BN, MINB>;
   static std::atomic<unsigned long long> attr_done{0};
-  if (int r = ensure_dyn_smem(igemm_kernel<BN, GEGLU, BF16>, CF::SMEM_BYTES, attr_done)) return r;
+  if (int r = ensure_dyn_smem(igemm_kernel<BN, MINB, GEGLU, BF16>, CF::SMEM_BYTES, attr_done)) return r;
   const int cl = p.cluster;
   const int tiles = ((p.num_m_tiles + cl - 1) / cl) * p.num_n_tiles;
   cudaLaunchConfig_t cfg;
@@ -498,7 +515,7 @@ static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorM
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  int clusters = num_sms() / cl;
+  int clusters = num_sms() * MINB / cl;     // persistent: MINB CTAs per SM
   if (cl > 1) {
     // a cluster's CTAs must fit inside one GPC: ask the driver how many clusters can be resident at once (cached per device)
     static std::atomic<int> max_clusters[64];
@@ -508,7 +525,7 @@ static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorM
     if (mc == 0) {
       cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<BN, GEGLU, BF16>, &cfg) != cudaSuccess || n < 1) {
+      if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<BN, MINB, GEGLU, BF16>, &cfg) != cudaSuccess || n < 1) {
         cudaGetLastError();
         n = 1;
       }
@@ -520,15 +537,15 @@ static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorM
   if (tiles < clusters) clusters = tiles;
   if (max_ctas > 0 && clusters > max_ctas / cl) clusters = max_ctas / cl > 0 ? max_ctas / cl : 1;
   cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, igemm_kernel<BN, GEGLU, BF16>, a, a2, b, p);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, igemm_kernel<BN, MINB, GEGLU, BF16>, a, a2, b, p);
   return e == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
 
-template <int BN, bool GEGLU>
+template <int BN, bool GEGLU, int MINB = 1>
 static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
                      int max_ctas, cudaStream_t stream) {
-  if (p.flags & AAB_F_BF16) return launch_t<BN, GEGLU, true>(a, a2, b, p, max_ctas, stream);
-  return launch_t<BN, GEGLU, false>(a, a2, b, p, max_ctas, stream);
+  if (p.flags & AAB_F_BF16) return launch_t<BN, MINB, GEGLU, true>(a, a2, b, p, max_ctas, stream);
+  return launch_t<BN, MINB, GEGLU, false>(a, a2, b, p, max_ctas, stream);
 }
 
 }  // namespace aab
@@ -567,6 +584,8 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
     if ((bn != 128 && bn != 256) || direct || d->residual || d->bias2 || d->act == AAB_ACT_SILU || d->out_scale != 1.0f)
       return AAB_ERR_ARG;
   }
+  const bool two_cta = (d->flags & AAB_F_TWO_CTA) != 0;
+  if (two_cta && (bn != 64 || geglu)) return AAB_ERR_ARG;   // the one width instantiated with MINB = 2
   if (d->num_taps < 1 || d->num_taps > AAB_MAX_TAPS) return AAB_ERR_ARG;
   if (d->kc % 8 != 0) return AAB_ERR_ARG;
   if (d->a2 && (d->kc1 % 64 != 0)) return AAB_ERR_ARG;
@@ -631,6 +650,7 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
     int r = make_tmap_16(&tmB, d->b, 3, dims, strides, box, is_bf16, 128);
     if (r) return r;
   }
+  if (two_cta) return launch_bn<64, false, 2>(tmA, tmA2, tmB, p, d->max_ctas, stream);
   if (geglu) {
     if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);
     return launch_bn<256, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);

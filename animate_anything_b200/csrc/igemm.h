@@ -16,6 +16,7 @@
 #define AAB_F_GEGLU 8     /* B rows [0,N/2) are values, [N/2,N) gates: out = value * gelu(gate), N/2 columns */
 #define AAB_F_PAIR 32     /* 256-column staged tiles on clusters of two CTAs sharing each weight tile (TMA multicast) */
 #define AAB_F_QUAD 16384  /* with AAB_F_PAIR: clusters of four (launches with fewer than 4 m-tiles use clusters of two) */
+#define AAB_F_TWO_CTA 64  /* two CTAs per SM (3-stage ring, 80 registers): block_n 64, not GEGLU */
 
 #ifdef __cplusplus
 extern "C" {
@@ -53,7 +54,7 @@ typedef struct AabIgemmDesc {
   int act;
   int flags;
   int block_n;              // 32 / 64 / 128 / 160 / 192 / 256 (GEGLU: 128 / 256)
-  int max_ctas;             // 0 = one CTA per SM
+  int max_ctas;             // 0 = one CTA per SM (two with AAB_F_TWO_CTA)
   float* colstats;          // optional [num_m_tiles][n_out][2] fp32: per m-tile column sums (sum, sum of squares) of the ROUNDED
                             // 16-bit outputs over the tile's valid rows -- the statistics of the GroupNorm that follows, taken
                             // where the data already is in registers (staged epilogues only), or NULL

@@ -13,7 +13,7 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, F_BF16, F_DIRECT, F_GEGLU, F_OUT_F32, F_PAIR, F_QUAD, F_SCALE_ACC,
-                   IgemmDesc)
+                   F_TWO_CTA, IgemmDesc)
 
 NUM_SMS = 132           # H100 SXM
 IGEMM_PROFILE = None     # bench.py sets this to a list to time every implicit-GEMM launch with CUDA events
@@ -136,6 +136,18 @@ def fit_block_n(n_out: int, m_tiles: int, sms: int = NUM_SMS) -> int:
     return max(w for w, c in cost.items() if c <= 1.05 * best)
 
 
+def pick_two_cta(n_out: int, m_tiles: int, k_total: int, taps: int, geglu: bool = False) -> int:
+    """Tile width of the two-CTAs-per-SM configuration for this launch, or 0 for the one-CTA path (`pick_block_n`).
+    With K <= 640 a tile is at most ten k-blocks of MMAs; with one CTA per SM its epilogue (bias, residual, stores) and
+    the ring refill for the next tile run with the tensor cores idle, and a second resident CTA fills that gap.  64-column
+    tiles only: the one width whose accumulators fit the 80 registers of two 384-thread CTAs (GEGLU needs 128).  Only with
+    at least one m-tile per resident CTA.  On an H100 at 700 W (tools/igemm_short_k.py, graph-replayed) every 1-tap
+    transformer linear of config 2 at K = 320 and 640 gains 12 - 43 % against the one-CTA widths (DESIGN.md section 6)."""
+    if geglu or taps != 1 or k_total > 640 or m_tiles < 2 * NUM_SMS or n_out < 320:
+        return 0
+    return 64
+
+
 def _fix_strides(dims, strides):
     """TMA wants non-zero, 16-byte-multiple strides even for extent-1 dims."""
     st = list(strides)
@@ -149,8 +161,10 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
           out: Optional[torch.Tensor] = None, ld_out: Optional[int] = None, *, bias=None, bias2=None, rows_per_bias2=1,
           residual=None, ld_res=None, act=ACT_NONE, out_scale=1.0, geglu=False, out_f32=False, a2=None, a2_dims=None,
           a2_strides=None, kc1=0, ld_b=None, b_batch=0, b_batch_stride=0, b_batch_dim=-1, block_n=None, direct=False,
-          max_ctas=0, out_rows=None, scale_acc=False, stats=False):
+          max_ctas=0, out_rows=None, scale_acc=False, stats=False, ctas_per_sm=None):
     """Generic launch of the implicit-GEMM kernel. `taps` is a list of 5-int offsets (channel, pix0..pix3).
+    `block_n` / `ctas_per_sm` (1, or 2 with `block_n=64`) override the tile width and the CTAs per SM that `pick_two_cta`
+    / `pick_block_n` choose from the shape; results are bit-identical whichever runs.
     `stats=True`: the output feeds a GroupNorm -- have the epilogue also write per-(128-row tile, column) sums / sums of
     squares of the rounded outputs (`out._aab_stats`, [m_tiles, n, 2] fp32) so that `groupnorm` can skip its statistics read.
     Silently not produced when the launch takes an epilogue that cannot (the consumer then runs the two-pass GroupNorm)."""
@@ -217,6 +231,11 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
     d.act = act
     flags = ((F_BF16 if bf else 0) | (F_GEGLU if geglu else 0) | (F_OUT_F32 if out_f32 else 0) | (F_DIRECT if direct else 0) |
              (F_SCALE_ACC if scale_acc else 0))
+    if block_n is None and ctas_per_sm is None:
+        block_n = pick_two_cta(n_out, m_tiles, kc * len(taps), len(taps), geglu) or None
+        ctas_per_sm = 2 if block_n else 1
+    if ctas_per_sm == 2:
+        flags |= F_TWO_CTA
     if block_n is None:
         if n_out < 64 and not geglu:
             # 32-column tiles only have the direct-store epilogue; an output that qualifies for the staged epilogue (and
@@ -252,7 +271,8 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         _lib.call("aab_igemm", C.byref(d), _stream())
         ev1.record()
         IGEMM_PROFILE.append({"rows": rows, "n": n, "k": kc * len(taps), "taps": len(taps), "block_n": block_n,
-                              "pair": bool(flags & F_PAIR), "geglu": geglu, "residual": residual is not None,
+                              "pair": bool(flags & F_PAIR), "two_cta": bool(flags & F_TWO_CTA), "geglu": geglu,
+                              "residual": residual is not None,
                               "flops": 2.0 * rows * n * kc * len(taps), "ev": (ev0, ev1)})
     else:
         _lib.call("aab_igemm", C.byref(d), _stream())
