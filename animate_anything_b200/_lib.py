@@ -13,9 +13,7 @@ LIB_PATH = os.environ.get("AAB_LIB_PATH") or os.path.join(_HERE, "libaab200.so")
 
 MAX_TAPS = 9
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_QUICK_GELU = 0, 1, 2, 3
-F_BF16, F_DIRECT, F_OUT_F32, F_GEGLU, F_SCALE_ACC, F_PAIR = 1, 2, 4, 8, 16, 32
-F_QUAD = 16384
-F_TWO_CTA = 64
+F_BF16, F_DIRECT, F_OUT_F32, F_GEGLU, F_SCALE_ACC, F_TWO_CTA = 1, 2, 4, 8, 16, 64
 
 
 class IgemmDesc(C.Structure):
@@ -32,7 +30,7 @@ class IgemmDesc(C.Structure):
         ("out", C.c_void_p), ("ld_out", C.c_long),
         ("bias", C.c_void_p), ("bias2", C.c_void_p), ("rows_per_bias2", C.c_int), ("ld_bias2", C.c_long),
         ("residual", C.c_void_p), ("ld_res", C.c_long),
-        ("out_scale", C.c_float), ("act", C.c_int), ("flags", C.c_int), ("block_n", C.c_int), ("max_ctas", C.c_int),
+        ("out_scale", C.c_float), ("act", C.c_int), ("flags", C.c_int), ("block_n", C.c_int),
         ("colstats", C.c_void_p),
     ]
 

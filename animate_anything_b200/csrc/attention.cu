@@ -55,7 +55,6 @@ template <bool BF16>
 __global__ void __launch_bounds__(FA_THREADS, 2)
 flash_attn_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const FaParams p) {
-  pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smQ = smem;
@@ -85,7 +84,6 @@ flash_attn_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (warp == 8) {
     if (elect_one()) {
@@ -214,7 +212,6 @@ constexpr int FA80_SMEM_BYTES = FA80_Q_BYTES + FA_KV_STAGES * 2 * FA80_KV_BYTES 
 template <bool BF16>
 __global__ void __launch_bounds__(FA_THREADS, 2)
 flash_attn_d80_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const FaParams p) {
-  pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smQ = smem;                                    // [5][128 x 16]
@@ -243,7 +240,6 @@ flash_attn_d80_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (warp == 8) {
     if (elect_one()) {
@@ -375,9 +371,9 @@ flash_attn_d80_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 // ------------------------------------------------------------------------------------------------ temporal
 // q/k/v rows of frame t of (b, position pos): base + ((b*T + t)*HW + pos)*ld + col0 + head*64
 // One warp per (b, pixel, head).  T <= 32 is far below the 64-row wgmma tile, so the two tiny GEMMs
-// (S = Q.K^T: 32x32x64, O = P.V: 32x64x32, T zero-padded to 32) run on warp-level mma.sync m16n8k16 with the online
-// softmax on the accumulator fragments (the S fragments are re-used as the A operand of P.V).  Q/K/V rows are gathered
-// with coalesced 8-byte loads into padded shared memory (row stride 144 B: conflict-free fragment loads).
+// (S = Q.K^T: 32x32x64, O = P.V: 32x64x32, T zero-padded to 32) run on warp-level mma.sync m16n8k16 with the
+// softmax on the accumulator fragments (the S fragments are re-used as the A operand of P.V).  Q/K/V rows sit in padded
+// shared memory (row stride 144 B: conflict-free fragment loads).
 template <bool BF16>
 __device__ __forceinline__ void mma_16816(float* c, const uint32_t* a, const uint32_t* b) {
   if (BF16)
@@ -393,155 +389,7 @@ __device__ __forceinline__ void mma_16816(float* c, const uint32_t* a, const uin
 constexpr int TA_ROW = 72;                    // halves per smem row (64 + 8 pad)
 constexpr int TA_WARP_HALVES = 3 * 32 * TA_ROW;
 
-template <bool BF16>
-__global__ void __launch_bounds__(128)
-temporal_attn_d64_kernel(const void* __restrict__ qkv, long ld, int q_col0, int k_col0, int v_col0, void* __restrict__ out,
-                         long ld_out, int B, int T, int HW, int heads, float scale) {
-  pdl_trigger();
-  pdl_wait();
-  extern __shared__ uint16_t sm16[];
-  const int w = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const long item = static_cast<long>(blockIdx.x) * 4 + w;
-  const long total = static_cast<long>(B) * HW * heads;
-  if (item >= total) return;
-  uint16_t* sQ = sm16 + static_cast<size_t>(w) * TA_WARP_HALVES;
-  uint16_t* sK = sQ + 32 * TA_ROW;
-  uint16_t* sV = sK + 32 * TA_ROW;
-  const int head = item % heads;
-  const long bp = item / heads;
-  const int pos = bp % HW;
-  const int b = bp / HW;
-  // gather: 16 lanes cover one 128-byte row (8 B per lane), two rows per iteration; rows >= T are zero
-  const int sub = lane & 15;
-  for (int t = lane >> 4; t < 32; t += 2) {
-    uint2 qu = make_uint2(0, 0), ku = make_uint2(0, 0), vu = make_uint2(0, 0);
-    if (t < T) {
-      const uint8_t* rowp = reinterpret_cast<const uint8_t*>(qkv) +
-                            (((static_cast<long>(b) * T + t) * HW + pos) * ld + head * 64 + sub * 4) * 2;
-      qu = *reinterpret_cast<const uint2*>(rowp + q_col0 * 2);
-      ku = *reinterpret_cast<const uint2*>(rowp + k_col0 * 2);
-      vu = *reinterpret_cast<const uint2*>(rowp + v_col0 * 2);
-    }
-    *reinterpret_cast<uint2*>(sQ + t * TA_ROW + sub * 4) = qu;
-    *reinterpret_cast<uint2*>(sK + t * TA_ROW + sub * 4) = ku;
-    *reinterpret_cast<uint2*>(sV + t * TA_ROW + sub * 4) = vu;
-  }
-  __syncwarp();
-  const int g = lane >> 2;      // fragment row group
-  const int t4 = lane & 3;      // fragment column pair
-  // ---------------- S = Q K^T  (2 m-tiles x 4 n-tiles)
-  float S[2][4][4];
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-    for (int nj = 0; nj < 4; ++nj)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) S[mi][nj][e] = 0.f;
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    uint32_t afr[2][4];
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi) {
-      const uint16_t* base = sQ + (16 * mi + g) * TA_ROW + 16 * kk + 2 * t4;
-      afr[mi][0] = *reinterpret_cast<const uint32_t*>(base);
-      afr[mi][1] = *reinterpret_cast<const uint32_t*>(base + 8 * TA_ROW);
-      afr[mi][2] = *reinterpret_cast<const uint32_t*>(base + 8);
-      afr[mi][3] = *reinterpret_cast<const uint32_t*>(base + 8 * TA_ROW + 8);
-    }
-#pragma unroll
-    for (int nj = 0; nj < 4; ++nj) {
-      uint32_t bfr[2];
-      const uint16_t* kb = sK + (8 * nj + g) * TA_ROW + 16 * kk + 2 * t4;
-      bfr[0] = *reinterpret_cast<const uint32_t*>(kb);
-      bfr[1] = *reinterpret_cast<const uint32_t*>(kb + 8);
-      mma_16816<BF16>(S[0][nj], afr[0], bfr);
-      mma_16816<BF16>(S[1][nj], afr[1], bfr);
-    }
-  }
-  // ---------------- softmax over the key axis (columns), rows (16 mi + g) and (16 mi + g + 8)
-  const float sl2 = scale * 1.4426950408889634f;
-  float inv_l[2][2];
-  uint32_t pfr[2][2][4];       // P as A fragments: [m-tile][k-step of 16 keys][4]
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {          // h = 0: row g, h = 1: row g + 8
-      float mx = -INFINITY;
-#pragma unroll
-      for (int nj = 0; nj < 4; ++nj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = 8 * nj + 2 * t4 + e;
-          float v = S[mi][nj][2 * h + e] * sl2;
-          v = (col < T) ? v : -INFINITY;
-          S[mi][nj][2 * h + e] = v;
-          mx = fmaxf(mx, v);
-        }
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      float l = 0.f;
-#pragma unroll
-      for (int nj = 0; nj < 4; ++nj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float pv = fast_exp2(S[mi][nj][2 * h + e] - mx);
-          S[mi][nj][2 * h + e] = pv;
-          l += pv;
-        }
-      l += __shfl_xor_sync(0xffffffffu, l, 1);
-      l += __shfl_xor_sync(0xffffffffu, l, 2);
-      inv_l[mi][h] = 1.0f / l;
-    }
-#pragma unroll
-    for (int k2 = 0; k2 < 2; ++k2) {
-      pfr[mi][k2][0] = pack2(S[mi][2 * k2][0], S[mi][2 * k2][1], BF16);
-      pfr[mi][k2][1] = pack2(S[mi][2 * k2][2], S[mi][2 * k2][3], BF16);
-      pfr[mi][k2][2] = pack2(S[mi][2 * k2 + 1][0], S[mi][2 * k2 + 1][1], BF16);
-      pfr[mi][k2][3] = pack2(S[mi][2 * k2 + 1][2], S[mi][2 * k2 + 1][3], BF16);
-    }
-  }
-  // ---------------- O = P V  (2 m-tiles x 8 n-tiles of d, 2 k-steps of 16 keys)
-  float O[2][8][4];
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-    for (int dj = 0; dj < 8; ++dj)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) O[mi][dj][e] = 0.f;
-#pragma unroll
-  for (int k2 = 0; k2 < 2; ++k2) {
-#pragma unroll
-    for (int dj = 0; dj < 8; ++dj) {
-      const uint16_t* vb = sV + (16 * k2 + 2 * t4) * TA_ROW + 8 * dj + g;
-      uint32_t bfr[2];
-      bfr[0] = static_cast<uint32_t>(vb[0]) | (static_cast<uint32_t>(vb[TA_ROW]) << 16);
-      bfr[1] = static_cast<uint32_t>(vb[8 * TA_ROW]) | (static_cast<uint32_t>(vb[9 * TA_ROW]) << 16);
-      mma_16816<BF16>(O[0][dj], pfr[0][k2], bfr);
-      mma_16816<BF16>(O[1][dj], pfr[1][k2], bfr);
-    }
-  }
-  // ---------------- normalise and store rows < T
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = 16 * mi + g + 8 * h;
-      if (row < T) {
-        const float il = inv_l[mi][h];
-        uint8_t* op = reinterpret_cast<uint8_t*>(out) +
-                      (((static_cast<long>(b) * T + row) * HW + pos) * ld_out + head * 64 + 2 * t4) * 2;
-#pragma unroll
-        for (int dj = 0; dj < 8; ++dj)
-          *reinterpret_cast<uint32_t*>(op + dj * 16) = pack2(O[mi][dj][2 * h] * il, O[mi][dj][2 * h + 1] * il, BF16);
-      }
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------ temporal v2
-// Same math as temporal_attn_d64_kernel (bit-identical results), restructured for HBM throughput.  Persistent warps walk the
-// (b, pixel, head) items;
+// Persistent warps walk the (b, pixel, head) items for HBM throughput:
 // the Q/K/V rows of the NEXT item are fetched with 16-byte cp.async copies straight into the second shared-memory buffer
 // (408 copies in flight per warp, no registers involved) while the current item is computed; the normalised output is
 // staged in shared memory and written with 16-byte stores (one 128-byte row per 8 lanes).
@@ -549,8 +397,6 @@ template <bool BF16>
 __global__ void __launch_bounds__(128)
 temporal_attn_d64_v2_kernel(const void* __restrict__ qkv, long ld, int q_col0, int k_col0, int v_col0,
                             void* __restrict__ out, long ld_out, int B, int T, int HW, int heads, float scale) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ uint16_t sm16[];
   const int w = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -752,8 +598,6 @@ temporal_attn_d64_long_kernel(const void* __restrict__ qkv, long ld, int q_col0,
   constexpr int NT = TP / 8;          // key n-tiles of S
   constexpr int KS = TP / 16;         // key k-steps of P.V
   constexpr int BUF = 3 * TP * TA_ROW;
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ uint16_t sm16[];
   const int w = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -957,11 +801,11 @@ extern "C" int aab_flash_attn_d64(const void* q, long ldq, long q_batch_stride, 
   if (is_bf16) {
     static std::atomic<unsigned long long> attr_b{0};
     if (int r = ensure_dyn_smem(flash_attn_d64_kernel<true>, FA_SMEM_BYTES, attr_b)) return r;
-    launch_k(flash_attn_d64_kernel<true>, grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
+    flash_attn_d64_kernel<true><<<grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
   } else {
     static std::atomic<unsigned long long> attr_h{0};
     if (int r = ensure_dyn_smem(flash_attn_d64_kernel<false>, FA_SMEM_BYTES, attr_h)) return r;
-    launch_k(flash_attn_d64_kernel<false>, grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream, tmQ, tmK, tmV, p);
+    flash_attn_d64_kernel<false><<<grid, dim3(FA_THREADS), FA_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
@@ -1012,11 +856,11 @@ extern "C" int aab_flash_attn_d80(const void* q, long ldq, long q_batch_stride, 
   if (is_bf16) {
     static std::atomic<unsigned long long> attr_b{0};
     if (int r = ensure_dyn_smem(flash_attn_d80_kernel<true>, FA80_SMEM_BYTES, attr_b)) return r;
-    launch_k(flash_attn_d80_kernel<true>, grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream, tmQ, tmKV, p);
+    flash_attn_d80_kernel<true><<<grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream>>>(tmQ, tmKV, p);
   } else {
     static std::atomic<unsigned long long> attr_h{0};
     if (int r = ensure_dyn_smem(flash_attn_d80_kernel<false>, FA80_SMEM_BYTES, attr_h)) return r;
-    launch_k(flash_attn_d80_kernel<false>, grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream, tmQ, tmKV, p);
+    flash_attn_d80_kernel<false><<<grid, dim3(FA_THREADS), FA80_SMEM_BYTES, stream>>>(tmQ, tmKV, p);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
@@ -1047,41 +891,22 @@ extern "C" int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k
     auto kern = tp == 64 ? (is_bf16 ? temporal_attn_d64_long_kernel<true, 64> : temporal_attn_d64_long_kernel<false, 64>)
                          : (is_bf16 ? temporal_attn_d64_long_kernel<true, 128> : temporal_attn_d64_long_kernel<false, 128>);
     if (int r = ensure_dyn_smem(kern, smem, attr)) return r;
-    launch_k(kern, dim3(grid), dim3(TAL_THREADS), smem, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw, heads,
+    kern<<<dim3(grid), dim3(TAL_THREADS), smem, stream>>>(qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw, heads,
              scale);
     return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
   }
-  static int use_v1 = -1;                 // AAB_TATTN_V1=1: the round-1 kernel (A/B measurements)
-  if (use_v1 < 0) {
-    const char* e = getenv("AAB_TATTN_V1");
-    use_v1 = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (!use_v1) {
-    const size_t smem2 = static_cast<size_t>(4) * 2 * TA_WARP_HALVES * sizeof(uint16_t);   // 108 KiB: double-buffered Q, K, V
-    static std::atomic<unsigned long long> a2t{0}, a2f{0};
-    if (int r = ensure_dyn_smem(temporal_attn_d64_v2_kernel<true>, static_cast<int>(smem2), a2t)) return r;
-    if (int r = ensure_dyn_smem(temporal_attn_d64_v2_kernel<false>, static_cast<int>(smem2), a2f)) return r;
-    long ctas = (total + 3) / 4;
-    const long cap = 2L * num_sms();                              // two 108 KiB CTAs per SM, persistent
-    const int grid2 = static_cast<int>(ctas < cap ? ctas : cap);
-    if (is_bf16)
-      launch_k(temporal_attn_d64_v2_kernel<true>, dim3(grid2), dim3(128), smem2, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw,
-                                                                       heads, scale);
-    else
-      launch_k(temporal_attn_d64_v2_kernel<false>, dim3(grid2), dim3(128), smem2, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw,
-                                                                        heads, scale);
-    return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
-  }
-  const int grid = static_cast<int>((total + 3) / 4);
-  const size_t smem = static_cast<size_t>(4) * TA_WARP_HALVES * sizeof(uint16_t);   // 54 KiB: Q, K, V padded to 32 rows
+  const size_t smem = static_cast<size_t>(4) * 2 * TA_WARP_HALVES * sizeof(uint16_t);   // 108 KiB: double-buffered Q, K, V
   static std::atomic<unsigned long long> attr_t{0}, attr_f{0};
-  if (int r = ensure_dyn_smem(temporal_attn_d64_kernel<true>, 65536, attr_t)) return r;
-  if (int r = ensure_dyn_smem(temporal_attn_d64_kernel<false>, 65536, attr_f)) return r;
+  if (int r = ensure_dyn_smem(temporal_attn_d64_v2_kernel<true>, static_cast<int>(smem), attr_t)) return r;
+  if (int r = ensure_dyn_smem(temporal_attn_d64_v2_kernel<false>, static_cast<int>(smem), attr_f)) return r;
+  const long ctas = (total + 3) / 4;
+  const long cap = 2L * num_sms();                              // two 108 KiB CTAs per SM, persistent
+  const int grid = static_cast<int>(ctas < cap ? ctas : cap);
   if (is_bf16)
-    launch_k(temporal_attn_d64_kernel<true>, dim3(grid), dim3(128), smem, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw,
-                                                                heads, scale);
+    temporal_attn_d64_v2_kernel<true><<<dim3(grid), dim3(128), smem, stream>>>(qkv, ld, q_col0, k_col0, v_col0, out, ld_out,
+             b, t, hw, heads, scale);
   else
-    launch_k(temporal_attn_d64_kernel<false>, dim3(grid), dim3(128), smem, stream, qkv, ld, q_col0, k_col0, v_col0, out, ld_out, b, t, hw,
-                                                                 heads, scale);
+    temporal_attn_d64_v2_kernel<false><<<dim3(grid), dim3(128), smem, stream>>>(qkv, ld, q_col0, k_col0, v_col0, out,
+             ld_out, b, t, hw, heads, scale);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }

@@ -56,8 +56,6 @@ __device__ __forceinline__ float u8_to_signed_unit(uint8_t v) {
 
 template <bool BF16>
 __global__ void __launch_bounds__(256) clip_image_prep_kernel(const ClipPrepParams p) {
-  pdl_trigger();
-  pdl_wait();
   const int row = blockIdx.x;                      // 0: class slot, 1 + patch index
   const int b = blockIdx.y;
   const int pp = p.patch * p.patch;
@@ -165,8 +163,8 @@ extern "C" int aab_clip_image_prep(const void* src, int src_type, long sb, long 
   p.ld_out = ld_out;
   const dim3 grid(1 + p.grid * p.grid, b);
   if (is_bf16)
-    launch_k(clip_image_prep_kernel<true>, grid, dim3(256), 0, stream, p);
+    clip_image_prep_kernel<true><<<grid, dim3(256), 0, stream>>>(p);
   else
-    launch_k(clip_image_prep_kernel<false>, grid, dim3(256), 0, stream, p);
+    clip_image_prep_kernel<false><<<grid, dim3(256), 0, stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }

@@ -144,58 +144,6 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- thread-block clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// every thread of every CTA of the cluster
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the copy of `bar` (same shared-memory offset) in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 ra;\n"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// wait that also orders after arrivals released by the other CTAs of the cluster
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  for (;;) {
-    uint32_t done;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (done) return;
-    if (++spins > (1u << 26)) __trap();
-  }
-}
-// TMA load delivered to the same shared-memory offset of every CTA in `cta_mask`; each destination's bytes are credited to
-// the barrier at the same offset in that CTA
-__device__ __forceinline__ void tma_load_3d_mcast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                  uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5, %6}], [%2], %3;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
-      "r"(c1), "r"(c2)
-      : "memory");
-}
-
 // ---------------------------------------------------------------- named barriers
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -263,43 +211,6 @@ inline int ensure_dyn_smem(Kernel kernel, int bytes, std::atomic<unsigned long l
   if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess) return AAB_ERR_CUDA;
   done.fetch_or(bit, std::memory_order_release);
   return AAB_OK;
-}
-
-// ---------------------------------------------------------------- programmatic dependent launch (PDL)
-// Every kernel of the path is launched with cudaLaunchAttributeProgrammaticStreamSerialization and follows one rule:
-//   pdl_trigger()  at the very top   -- the NEXT kernel of the stream may be scheduled as soon as every CTA of this grid
-//                                       has started (its CTAs take the SM resources this grid frees while draining);
-//   pdl_wait()     before the first global-memory access (read OR write) -- blocks until the PREVIOUS grid has completed
-//                                       and its memory is visible.
-// So only set-up work (barrier init, descriptor prefetch, index math) overlaps the predecessor's tail; data hazards are
-// impossible by construction.  Off by default (launches carry no attribute and both calls are no-ops); AAB_PDL=1 enables it.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-inline bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("AAB_PDL");
-    on = (e && e[0] == '1') ? 1 : 0;
-  }
-  return on != 0;
-}
-
-// kernel<<<grid, block, smem, stream>>>(args...) with the PDL attribute (and an optional cluster dimension)
-template <typename... P, typename... A>
-inline cudaError_t launch_k(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A&&... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<P>(args)...);
 }
 
 // ---------------------------------------------------------------- numeric helpers

@@ -16,8 +16,6 @@ template <bool BF16>
 __global__ void unet_in_assemble_kernel(const void* __restrict__ sample, Strides5 ss, const void* __restrict__ cond,
                                         Strides5 cs, const void* __restrict__ mask, Strides5 ms, int mask_batch,
                                         void* __restrict__ out, int B, int T, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * T * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -53,8 +51,6 @@ __global__ void unet_in_assemble_kernel(const void* __restrict__ sample, Strides
 template <bool BF16>
 __global__ void unet_out_finalize_kernel(const float* __restrict__ y, int ldc, void* __restrict__ out, int B, int T,
                                          int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const int F = T - 1;
   const long total = static_cast<long>(B) * 4 * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -76,8 +72,6 @@ __global__ void unet_out_finalize_kernel(const float* __restrict__ y, int ldc, v
 // (models/unet_3d_condition_mask.py:146,156,408,415): out[b, j] = cos(t * w_j) for j < half, sin(t * w_{j-half}) after.
 template <bool BF16>
 __global__ void timestep_embed_kernel(const float* __restrict__ t, int t_count, void* __restrict__ out, int B, int dim) {
-  pdl_trigger();
-  pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * dim) return;
   const int b = i / dim;
@@ -97,8 +91,6 @@ template <bool BF16>
 __global__ void embed_tokens_kernel(const long long* __restrict__ ids, const uint4* __restrict__ tok,
                                     const uint4* __restrict__ pos, uint4* __restrict__ out, long rows, int L, int V8,
                                     int vocab) {
-  pdl_trigger();
-  pdl_wait();
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= rows * V8) return;
   const long r = i / V8;
@@ -123,8 +115,6 @@ __global__ void embed_tokens_kernel(const long long* __restrict__ ids, const uin
 // GEGLU fallback: out[r, j] = x[r, j] * gelu(x[r, nh + j])   (diffusers GEGLU.forward)
 template <bool BF16>
 __global__ void geglu_kernel(const void* __restrict__ x, long ldx, void* __restrict__ out, long ldo, long rows, int nh) {
-  pdl_trigger();
-  pdl_wait();
   const long total = rows * (nh / 8);
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -146,8 +136,6 @@ __global__ void geglu_kernel(const void* __restrict__ x, long ldx, void* __restr
 
 // nearest-neighbour 2x upsample on channels-last [N, H, W, C] -> [N, 2H, 2W, C]  (diffusers Upsample2D, F.interpolate)
 __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, long n, int H, int W, int V) {
-  pdl_trigger();
-  pdl_wait();
   const long total = n * 2 * H * 2 * W * V;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -165,8 +153,6 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
 // computes it).  Reached when the latent size is not a multiple of 8 (models/unet_3d_condition_mask.py:377-383,486-491).
 __global__ void upsample_nearest_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, long n, int H, int W, int OH,
                                         int OW, int V) {
-  pdl_trigger();
-  pdl_wait();
   const long total = n * OH * OW * V;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -188,8 +174,6 @@ __global__ void upsample_nearest_kernel(const uint4* __restrict__ x, uint4* __re
 // zero padding at the bottom / right: [N, H, W, C] -> [N, H + ph, W + pw, C].  Makes an odd-sized activation even so that the
 // stride-2 convolution can use its space-to-depth view; the added zeros are exactly the conv's own zero padding.
 __global__ void pad_br_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, long n, int H, int W, int PH, int PW, int V) {
-  pdl_trigger();
-  pdl_wait();
   const long total = n * PH * PW * V;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -207,8 +191,6 @@ __global__ void pad_br_kernel(const uint4* __restrict__ x, uint4* __restrict__ y
 // strided 16-bit copy of a [rows, cols] block (used for K/V^T staging and channel concat fallbacks)
 __global__ void copy2d_kernel(const uint16_t* __restrict__ src, long lds, uint16_t* __restrict__ dst, long ldd, long rows,
                               int cols) {
-  pdl_trigger();
-  pdl_wait();
   const long total = rows * cols;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -219,8 +201,6 @@ __global__ void copy2d_kernel(const uint16_t* __restrict__ src, long lds, uint16
 
 // same copy in 16-byte units (cols, both row strides and both base addresses multiples of 8 elements)
 __global__ void copy2d_v8_kernel(const uint4* __restrict__ src, long lds8, uint4* __restrict__ dst, long ldd8, long rows, int cols8) {
-  pdl_trigger();
-  pdl_wait();
   const long total = rows * cols8;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -232,8 +212,6 @@ __global__ void copy2d_v8_kernel(const uint4* __restrict__ src, long lds8, uint4
 // out[0:n16] = out[n16:2*n16] = src (16-byte units): duplicates the rows of the unconditional half for the text half when
 // the CFG pair shares its prefix (see UNet3DConditionModel.forward, `_cfg_shared_prefix`)
 __global__ void dup_rows_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, long n16) {
-  pdl_trigger();
-  pdl_wait();
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n16) return;
   const uint4 v = __ldg(src + i);
@@ -245,8 +223,6 @@ __global__ void dup_rows_kernel(const uint4* __restrict__ src, uint4* __restrict
 // (ldd = rows rounded up to a multiple of 8 so that the result can be a TMA operand when rows % 8 != 0)
 __global__ void transpose_kernel(const uint16_t* __restrict__ src, long lds, long src_batch, uint16_t* __restrict__ dst,
                                  int rows, int cols, int ldd) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ uint16_t tile[32][33];
   const int b = blockIdx.z;
   const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
@@ -274,8 +250,6 @@ __global__ void cfg_step_kernel(const float* __restrict__ eps, int ldc, int cfg,
                                 const void* __restrict__ x, void* __restrict__ x_out, float* __restrict__ x0_hist,
                                 const float* __restrict__ coef, const int* __restrict__ step_idx, int n, int F, int H,
                                 int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(n) * 4 * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -314,8 +288,6 @@ __global__ void cfg_step_kernel(const float* __restrict__ eps, int ldc, int cfg,
 template <bool BF16>
 __global__ void image_to_nhwc8_kernel(const void* __restrict__ img, long sn, long sc, long sy, long sx,
                                       void* __restrict__ out, long N, int C, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = N * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -335,8 +307,6 @@ __global__ void image_to_nhwc8_kernel(const void* __restrict__ img, long sn, lon
 template <bool BF16>
 __global__ void image_to_nhwc16_kernel(const void* __restrict__ img, long sn, long sc, long sy, long sx,
                                        void* __restrict__ out, long N, int C, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = N * H * W * 2;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -365,8 +335,6 @@ __global__ void image_to_nhwc16_kernel(const void* __restrict__ img, long sn, lo
 template <bool BF16>
 __global__ void add_rowvec_kernel(const void* x, long ldx, void* out, long ldo, const float* __restrict__ vec, long ldv, long rows,
                                   int cols, long rows_per_vec, int mod, int mode, int mod2) {
-  pdl_trigger();
-  pdl_wait();
   const int V = cols >> 3;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= rows * V) return;
@@ -402,8 +370,6 @@ __global__ void add_rowvec_kernel(const void* x, long ldx, void* out, long ldo, 
 template <bool BF16>
 __global__ void axpby_kernel(const uint4* __restrict__ x, const uint4* __restrict__ y, uint4* __restrict__ out, long n16,
                              float a, float b) {
-  pdl_trigger();
-  pdl_wait();
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n16) return;
   const uint4 ux = __ldg(x + i), uy = __ldg(y + i);
@@ -423,8 +389,6 @@ __global__ void axpby_kernel(const uint4* __restrict__ x, const uint4* __restric
 // (UNetSpatioTemporalConditionModel.forward tail: sample.reshape(batch, frames, C, H, W))
 template <bool BF16>
 __global__ void svd_out_finalize_kernel(const float* __restrict__ y, int ldc, void* __restrict__ out, long BF, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = BF * 4 * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -449,8 +413,6 @@ template <bool BF16>
 __global__ void svd_in_assemble_kernel(const void* __restrict__ x, const void* __restrict__ img_lat, const void* __restrict__ mask,
                                        float inv_scale, void* __restrict__ out, int B, int F, int H, int W, int cfg, long cond_hs,
                                        long cond_bs, long cond_fs, int zero_uncond, long mask_bs, long mask_fs) {
-  pdl_trigger();
-  pdl_wait();
   const long per_half = static_cast<long>(B) * F * H * W;
   const long total = per_half * (cfg ? 2 : 1) * 2;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -498,8 +460,6 @@ template <bool BF16>
 __global__ void svd_cfg_euler_step_kernel(const float* __restrict__ pred, int ldc, int cfg, const float* __restrict__ gs,
                                           const void* __restrict__ x, void* __restrict__ x_out, float sigma, float sigma_next,
                                           int B, int F, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * F * 4 * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -535,8 +495,6 @@ template <bool BF16>
 __global__ void vae_enc_finalize_kernel(const void* __restrict__ mom, int ldm, const float* __restrict__ wq /*[8][8]*/,
                                         const float* __restrict__ bq, float scale, void* __restrict__ out, int B, int F,
                                         int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -565,8 +523,6 @@ __global__ void vae_enc_finalize_kernel(const void* __restrict__ mom, int ldm, c
 template <bool BF16>
 __global__ void vae_dec_in_kernel(const void* __restrict__ lat, float inv_scale, const float* __restrict__ wp /*[4][4]*/,
                                   const float* __restrict__ bp, void* __restrict__ out, int B, int F, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -601,8 +557,6 @@ __global__ void vae_dec_in_kernel(const void* __restrict__ lat, float inv_scale,
 template <bool BF16>
 __global__ void vae_dec_finalize_kernel(const float* __restrict__ y, int ldc, float* __restrict__ out, int B, int F,
                                         int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * 3 * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -627,8 +581,6 @@ __global__ void vae_dec_finalize_kernel(const float* __restrict__ y, int ldc, fl
 template <bool BF16, bool RINT>
 __global__ void vae_dec_finalize_u8_kernel(const float* __restrict__ y, int ldc, uint8_t* __restrict__ out, int B, int F,
                                            int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(F) * H * B * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -656,8 +608,6 @@ __global__ void vae_dec_finalize_u8_kernel(const float* __restrict__ y, int ldc,
 template <bool BF16>
 __global__ void add_noise_kernel(const void* __restrict__ x0, const void* __restrict__ noise, float sa, float sb,
                                  void* __restrict__ out, long bc, int F, int FX, long HW) {
-  pdl_trigger();
-  pdl_wait();
   const long total = bc * F * HW;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -675,8 +625,6 @@ __global__ void add_noise_kernel(const void* __restrict__ x0, const void* __rest
 // fp32 -> 16-bit convert (weights / small tensors)
 template <bool BF16>
 __global__ void cast_f32_kernel(const float* __restrict__ x, void* __restrict__ y, long n) {
-  pdl_trigger();
-  pdl_wait();
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) store_elem(y, i, x[i], BF16);
 }
@@ -688,8 +636,6 @@ __global__ void cast_f32_kernel(const float* __restrict__ x, void* __restrict__ 
 template <bool BF16>
 __global__ void video_f32_to_nhwc8_kernel(const float* __restrict__ v, long sb, long sc, long sf, long sy, long sx,
                                           void* __restrict__ out, int B, int C, int F, int H, int W) {
-  pdl_trigger();
-  pdl_wait();
   const long total = static_cast<long>(B) * F * H * W;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -714,8 +660,6 @@ __global__ void video_f32_to_nhwc8_kernel(const float* __restrict__ v, long sb, 
 //   fg    = round16(round16(v + 1) * 127.5)  -> float -> clip(0, 255) -> truncate   (numpy astype(uint8))
 template <bool BF16>
 __global__ void rgba_finalize_u8_kernel(const float* __restrict__ y, int ldc, uint8_t* __restrict__ out, long pixels) {
-  pdl_trigger();
-  pdl_wait();
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= pixels) return;
   const float* src = y + i * ldc;
@@ -736,8 +680,6 @@ __global__ void rgba_finalize_u8_kernel(const float* __restrict__ y, int ldc, ui
 // dst [rows, ldd] = src [rows, cols] with columns cols..dcols-1 zero: widens a 32-channel activation to the 64-channel K
 // block of the stride-2 implicit GEMM (UNet384 level-0 Downsample2D, LatentTransparencyOffsetEncoder 32 -> 64 conv).
 __global__ void pad_cols_kernel(const uint4* __restrict__ src, long lds8, uint4* __restrict__ dst, long rows, int cols8, int dcols8) {
-  pdl_trigger();
-  pdl_wait();
   const long total = rows * dcols8;
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -764,10 +706,10 @@ extern "C" int aab_unet_in_assemble(const void* sample, const long* s_strides /*
   if (mask) ms = Strides5{m_strides[0], m_strides[1], m_strides[2], m_strides[3], m_strides[4]};
   const long total = static_cast<long>(b) * t * h * w;
   if (is_bf16)
-    launch_k(unet_in_assemble_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, sample, ss, cond, cs, mask, ms,
+    unet_in_assemble_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(sample, ss, cond, cs, mask, ms,
                                                                             mask_batch > 0 ? mask_batch : 1, out, b, t, h, w);
   else
-    launch_k(unet_in_assemble_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, sample, ss, cond, cs, mask, ms,
+    unet_in_assemble_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(sample, ss, cond, cs, mask, ms,
                                                                              mask_batch > 0 ? mask_batch : 1, out, b, t, h, w);
   AAB_LAUNCH_RET();
 }
@@ -776,8 +718,8 @@ extern "C" int aab_unet_out_finalize(const float* y, int ldc, void* out, int b, 
                                      void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const long total = static_cast<long>(b) * 4 * (t - 1) * h * w;
-  if (is_bf16) launch_k(unet_out_finalize_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, b, t, h, w);
-  else launch_k(unet_out_finalize_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, b, t, h, w);
+  if (is_bf16) unet_out_finalize_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, b, t, h, w);
+  else unet_out_finalize_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, b, t, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -787,8 +729,8 @@ extern "C" int aab_timestep_embed(const float* t, int t_count, void* out, int b,
   // index out of bounds (the reference raises a broadcast error in that case)
   if (!t || !out || (dim & 1) || t_count < 1 || b < 1 || (b % t_count) != 0) return AAB_ERR_ARG;
   const long total = static_cast<long>(b) * dim;
-  if (is_bf16) launch_k(timestep_embed_kernel<true>, dim3(AAB_GRID(total, 128)), dim3(128), 0, stream, t, t_count, out, b, dim);
-  else launch_k(timestep_embed_kernel<false>, dim3(AAB_GRID(total, 128)), dim3(128), 0, stream, t, t_count, out, b, dim);
+  if (is_bf16) timestep_embed_kernel<true><<<dim3(AAB_GRID(total, 128)), dim3(128), 0, stream>>>(t, t_count, out, b, dim);
+  else timestep_embed_kernel<false><<<dim3(AAB_GRID(total, 128)), dim3(128), 0, stream>>>(t, t_count, out, b, dim);
   AAB_LAUNCH_RET();
 }
 
@@ -798,11 +740,11 @@ extern "C" int aab_embed_tokens(const long long* ids, const void* tok_emb, const
   if (!ids || !tok_emb || !pos_emb || !out || (c % 8) || seq_len < 1 || vocab < 1) return AAB_ERR_ARG;
   const long total = rows * (c / 8);
   if (is_bf16)
-    launch_k(embed_tokens_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, 
+    embed_tokens_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(
         ids, reinterpret_cast<const uint4*>(tok_emb), reinterpret_cast<const uint4*>(pos_emb),
         reinterpret_cast<uint4*>(out), rows, seq_len, c / 8, vocab);
   else
-    launch_k(embed_tokens_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, 
+    embed_tokens_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(
         ids, reinterpret_cast<const uint4*>(tok_emb), reinterpret_cast<const uint4*>(pos_emb),
         reinterpret_cast<uint4*>(out), rows, seq_len, c / 8, vocab);
   AAB_LAUNCH_RET();
@@ -812,8 +754,8 @@ extern "C" int aab_geglu(const void* x, long ldx, void* out, long ldo, long rows
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if ((nh % 8) || (ldx % 8) || (ldo % 8)) return AAB_ERR_ARG;
   const long total = rows * (nh / 8);
-  if (is_bf16) launch_k(geglu_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, ldx, out, ldo, rows, nh);
-  else launch_k(geglu_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, ldx, out, ldo, rows, nh);
+  if (is_bf16) geglu_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, ldx, out, ldo, rows, nh);
+  else geglu_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, ldx, out, ldo, rows, nh);
   AAB_LAUNCH_RET();
 }
 
@@ -821,7 +763,7 @@ extern "C" int aab_upsample2x(const void* x, void* y, long n, int h, int w, int 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (c % 8) return AAB_ERR_ARG;
   const long total = n * 2 * h * 2 * w * (c / 8);
-  launch_k(upsample2x_kernel, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x),
+  upsample2x_kernel<<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(x),
                                                                reinterpret_cast<uint4*>(y), n, h, w, c / 8);
   AAB_LAUNCH_RET();
 }
@@ -830,7 +772,7 @@ extern "C" int aab_upsample_nearest(const void* x, void* y, long n, int h, int w
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || (c % 8) || h < 1 || w < 1 || oh < 1 || ow < 1) return AAB_ERR_ARG;
   const long total = n * oh * ow * (c / 8);
-  launch_k(upsample_nearest_kernel, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x),
+  upsample_nearest_kernel<<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(x),
                                                                      reinterpret_cast<uint4*>(y), n, h, w, oh, ow, c / 8);
   AAB_LAUNCH_RET();
 }
@@ -839,7 +781,7 @@ extern "C" int aab_pad_br(const void* x, void* y, long n, int h, int w, int ph, 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || (c % 8) || ph < h || pw < w) return AAB_ERR_ARG;
   const long total = n * ph * pw * (c / 8);
-  launch_k(pad_br_kernel, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), n,
+  pad_br_kernel<<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), n,
                                                            h, w, ph, pw, c / 8);
   AAB_LAUNCH_RET();
 }
@@ -849,11 +791,11 @@ extern "C" int aab_copy2d(const void* src, long lds, void* dst, long ldd, long r
   const long total = rows * cols;
   if (cols % 8 == 0 && lds % 8 == 0 && ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(src) % 16) == 0 &&
       (reinterpret_cast<uintptr_t>(dst) % 16) == 0) {
-    launch_k(copy2d_v8_kernel, dim3(AAB_GRID(total / 8, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(src), lds / 8,
+    copy2d_v8_kernel<<<dim3(AAB_GRID(total / 8, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(src), lds / 8,
              reinterpret_cast<uint4*>(dst), ldd / 8, rows, cols / 8);
     AAB_LAUNCH_RET();
   }
-  launch_k(copy2d_kernel, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint16_t*>(src), lds,
+  copy2d_kernel<<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint16_t*>(src), lds,
                                                           reinterpret_cast<uint16_t*>(dst), ldd, rows, cols);
   AAB_LAUNCH_RET();
 }
@@ -862,7 +804,7 @@ extern "C" int aab_dup_rows(const void* src, void* dst, long bytes, void* stream
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!src || !dst || (bytes % 16)) return AAB_ERR_ARG;
   const long n16 = bytes / 16;
-  launch_k(dup_rows_kernel, dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(src),
+  dup_rows_kernel<<<dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(src),
                                                          reinterpret_cast<uint4*>(dst), n16);
   AAB_LAUNCH_RET();
 }
@@ -872,7 +814,7 @@ extern "C" int aab_transpose(const void* src, long lds, long src_batch, void* ds
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!src || !dst || ldd < rows) return AAB_ERR_ARG;
   dim3 grid((cols + 31) / 32, (ldd + 31) / 32, nb);
-  launch_k(transpose_kernel, dim3(grid), dim3(dim3(32, 8)), 0, stream, reinterpret_cast<const uint16_t*>(src), lds, src_batch,
+  transpose_kernel<<<dim3(grid), dim3(dim3(32, 8)), 0, stream>>>(reinterpret_cast<const uint16_t*>(src), lds, src_batch,
                                                      reinterpret_cast<uint16_t*>(dst), rows, cols, ldd);
   AAB_LAUNCH_RET();
 }
@@ -884,10 +826,10 @@ extern "C" int aab_cfg_scheduler_step(const float* eps, int ldc, int cfg, float 
   if (!eps || !x || !x_out || !coef) return AAB_ERR_ARG;
   const long total = static_cast<long>(n) * 4 * f * h * w;
   if (is_bf16)
-    launch_k(cfg_step_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, eps, ldc, cfg, guidance, x, x_out, x0_hist, coef,
+    cfg_step_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(eps, ldc, cfg, guidance, x, x_out, x0_hist, coef,
                                                                     step_idx, n, f, h, w);
   else
-    launch_k(cfg_step_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, eps, ldc, cfg, guidance, x, x_out, x0_hist, coef,
+    cfg_step_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(eps, ldc, cfg, guidance, x, x_out, x0_hist, coef,
                                                                      step_idx, n, f, h, w);
   AAB_LAUNCH_RET();
 }
@@ -897,8 +839,8 @@ extern "C" int aab_image_to_nhwc8(const void* img, long sn, long sc, long sy, lo
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (c > 8) return AAB_ERR_ARG;
   const long total = n * h * w;
-  if (is_bf16) launch_k(image_to_nhwc8_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, img, sn, sc, sy, sx, out, n, c, h, w);
-  else launch_k(image_to_nhwc8_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, img, sn, sc, sy, sx, out, n, c, h, w);
+  if (is_bf16) image_to_nhwc8_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(img, sn, sc, sy, sx, out, n, c, h, w);
+  else image_to_nhwc8_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(img, sn, sc, sy, sx, out, n, c, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -907,8 +849,8 @@ extern "C" int aab_image_to_nhwc16(const void* img, long sn, long sc, long sy, l
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!img || !out || c > 16 || c < 1) return AAB_ERR_ARG;
   const long total = n * h * w * 2;
-  if (is_bf16) launch_k(image_to_nhwc16_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, img, sn, sc, sy, sx, out, n, c, h, w);
-  else launch_k(image_to_nhwc16_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, img, sn, sc, sy, sx, out, n, c, h, w);
+  if (is_bf16) image_to_nhwc16_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(img, sn, sc, sy, sx, out, n, c, h, w);
+  else image_to_nhwc16_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(img, sn, sc, sy, sx, out, n, c, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -920,10 +862,10 @@ extern "C" int aab_add_rowvec(const void* x, long ldx, void* out, long ldo, cons
     return AAB_ERR_ARG;
   const long total = rows * (cols / 8);
   if (is_bf16)
-    launch_k(add_rowvec_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, ldx, out, ldo, vec, ldv, rows, cols, rows_per_vec, mod,
+    add_rowvec_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, ldx, out, ldo, vec, ldv, rows, cols, rows_per_vec, mod,
                                                                      mode, mod2);
   else
-    launch_k(add_rowvec_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, ldx, out, ldo, vec, ldv, rows, cols, rows_per_vec, mod,
+    add_rowvec_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, ldx, out, ldo, vec, ldv, rows, cols, rows_per_vec, mod,
                                                                       mode, mod2);
   AAB_LAUNCH_RET();
 }
@@ -933,11 +875,11 @@ extern "C" int aab_axpby(const void* x, const void* y, void* out, long n_elems, 
   if (!x || !y || !out || (n_elems % 8)) return AAB_ERR_ARG;
   const long n16 = n_elems / 8;
   if (is_bf16)
-    launch_k(axpby_kernel<true>, dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x),
+    axpby_kernel<true><<<dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(x),
                                                                  reinterpret_cast<const uint4*>(y),
                                                                  reinterpret_cast<uint4*>(out), n16, a, b);
   else
-    launch_k(axpby_kernel<false>, dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x),
+    axpby_kernel<false><<<dim3(AAB_GRID(n16, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(x),
                                                                   reinterpret_cast<const uint4*>(y),
                                                                   reinterpret_cast<uint4*>(out), n16, a, b);
   AAB_LAUNCH_RET();
@@ -947,8 +889,8 @@ extern "C" int aab_svd_out_finalize(const float* y, int ldc, void* out, long bf,
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!y || !out || ldc < 4) return AAB_ERR_ARG;
   const long total = bf * 4 * h * w;
-  if (is_bf16) launch_k(svd_out_finalize_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, bf, h, w);
-  else launch_k(svd_out_finalize_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, bf, h, w);
+  if (is_bf16) svd_out_finalize_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, bf, h, w);
+  else svd_out_finalize_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, bf, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -958,8 +900,8 @@ extern "C" int aab_svd_in_assemble(const void* x, const void* img_lat, const voi
   if (!x || !img_lat || !mask || !out) return AAB_ERR_ARG;
   const long total = static_cast<long>(b) * f * h * w * (cfg ? 2 : 1) * 2;
   const long hw4 = 4L * h * w;
-  if (is_bf16) launch_k(svd_in_assemble_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, img_lat, mask, inv_scale, out, b, f, h, w, cfg, 0L, hw4, 0L, 1, 0L, 0L);
-  else launch_k(svd_in_assemble_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, img_lat, mask, inv_scale, out, b, f, h, w, cfg, 0L, hw4, 0L, 1, 0L, 0L);
+  if (is_bf16) svd_in_assemble_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, img_lat, mask, inv_scale, out, b, f, h, w, cfg, 0L, hw4, 0L, 1, 0L, 0L);
+  else svd_in_assemble_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, img_lat, mask, inv_scale, out, b, f, h, w, cfg, 0L, hw4, 0L, 1, 0L, 0L);
   AAB_LAUNCH_RET();
 }
 
@@ -970,8 +912,8 @@ extern "C" int aab_svd_in_assemble_frames(const void* x, const void* cond, long 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !cond || !out) return AAB_ERR_ARG;
   const long total = static_cast<long>(b) * f * h * w * (cfg ? 2 : 1) * 2;
-  if (is_bf16) launch_k(svd_in_assemble_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, cond, mask, inv_scale, out, b, f, h, w, cfg, cond_half_stride, cond_batch_stride, cond_frame_stride, zero_uncond, mask_batch_stride, mask_frame_stride);
-  else launch_k(svd_in_assemble_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x, cond, mask, inv_scale, out, b, f, h, w, cfg, cond_half_stride, cond_batch_stride, cond_frame_stride, zero_uncond, mask_batch_stride, mask_frame_stride);
+  if (is_bf16) svd_in_assemble_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, cond, mask, inv_scale, out, b, f, h, w, cfg, cond_half_stride, cond_batch_stride, cond_frame_stride, zero_uncond, mask_batch_stride, mask_frame_stride);
+  else svd_in_assemble_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x, cond, mask, inv_scale, out, b, f, h, w, cfg, cond_half_stride, cond_batch_stride, cond_frame_stride, zero_uncond, mask_batch_stride, mask_frame_stride);
   AAB_LAUNCH_RET();
 }
 
@@ -981,10 +923,10 @@ extern "C" int aab_svd_cfg_euler_step(const float* pred, int ldc, int cfg, const
   if (!pred || !x || !x_out || (cfg && !gs) || ldc < 4 || sigma <= 0.f) return AAB_ERR_ARG;
   const long total = static_cast<long>(b) * f * 4 * h * w;
   if (is_bf16)
-    launch_k(svd_cfg_euler_step_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, pred, ldc, cfg, gs, x, x_out, sigma, sigma_next, b,
+    svd_cfg_euler_step_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(pred, ldc, cfg, gs, x, x_out, sigma, sigma_next, b,
                                                                              f, h, w);
   else
-    launch_k(svd_cfg_euler_step_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, pred, ldc, cfg, gs, x, x_out, sigma, sigma_next, b,
+    svd_cfg_euler_step_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(pred, ldc, cfg, gs, x, x_out, sigma, sigma_next, b,
                                                                               f, h, w);
   AAB_LAUNCH_RET();
 }
@@ -993,8 +935,8 @@ extern "C" int aab_vae_enc_finalize(const void* mom, int ldm, const float* wq, c
                                     int b, int f, int h, int w, int is_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const long total = static_cast<long>(b) * f * h * w;
-  if (is_bf16) launch_k(vae_enc_finalize_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, mom, ldm, wq, bq, scale, out, b, f, h, w);
-  else launch_k(vae_enc_finalize_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, mom, ldm, wq, bq, scale, out, b, f, h, w);
+  if (is_bf16) vae_enc_finalize_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(mom, ldm, wq, bq, scale, out, b, f, h, w);
+  else vae_enc_finalize_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(mom, ldm, wq, bq, scale, out, b, f, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -1002,8 +944,8 @@ extern "C" int aab_vae_dec_in(const void* lat, float inv_scale, const float* wp,
                               int h, int w, int is_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const long total = static_cast<long>(b) * f * h * w;
-  if (is_bf16) launch_k(vae_dec_in_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, lat, inv_scale, wp, bp, out, b, f, h, w);
-  else launch_k(vae_dec_in_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, lat, inv_scale, wp, bp, out, b, f, h, w);
+  if (is_bf16) vae_dec_in_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(lat, inv_scale, wp, bp, out, b, f, h, w);
+  else vae_dec_in_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(lat, inv_scale, wp, bp, out, b, f, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -1011,8 +953,8 @@ extern "C" int aab_vae_dec_finalize(const float* y, int ldc, float* out, int b, 
                                     void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const long total = static_cast<long>(b) * 3 * f * h * w;
-  if (is_bf16) launch_k(vae_dec_finalize_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, b, f, h, w);
-  else launch_k(vae_dec_finalize_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, y, ldc, out, b, f, h, w);
+  if (is_bf16) vae_dec_finalize_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, b, f, h, w);
+  else vae_dec_finalize_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(y, ldc, out, b, f, h, w);
   AAB_LAUNCH_RET();
 }
 
@@ -1025,10 +967,10 @@ extern "C" int aab_vae_dec_finalize_u8(const float* y, int ldc, void* out, int b
   uint8_t* o = reinterpret_cast<uint8_t*>(out);
   const dim3 grid(AAB_GRID(total, 256)), block(256);
   switch (is_bf16) {
-    case 0: launch_k(vae_dec_finalize_u8_kernel<false, false>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
-    case 1: launch_k(vae_dec_finalize_u8_kernel<true, false>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
-    case 2: launch_k(vae_dec_finalize_u8_kernel<false, true>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
-    default: launch_k(vae_dec_finalize_u8_kernel<true, true>, grid, block, 0, stream, y, ldc, o, b, f, h, w); break;
+    case 0: vae_dec_finalize_u8_kernel<false, false><<<grid, block, 0, stream>>>(y, ldc, o, b, f, h, w); break;
+    case 1: vae_dec_finalize_u8_kernel<true, false><<<grid, block, 0, stream>>>(y, ldc, o, b, f, h, w); break;
+    case 2: vae_dec_finalize_u8_kernel<false, true><<<grid, block, 0, stream>>>(y, ldc, o, b, f, h, w); break;
+    default: vae_dec_finalize_u8_kernel<true, true><<<grid, block, 0, stream>>>(y, ldc, o, b, f, h, w); break;
   }
   AAB_LAUNCH_RET();
 }
@@ -1038,15 +980,15 @@ extern "C" int aab_add_noise(const void* x0, const void* noise, float sa, float 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x0 || !noise || !out || bc < 1 || f < 1 || hw < 1 || (fx != 1 && fx != f)) return AAB_ERR_ARG;
   const long total = bc * f * hw;
-  if (is_bf16) launch_k(add_noise_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x0, noise, sa, sb, out, bc, f, fx, hw);
-  else launch_k(add_noise_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, x0, noise, sa, sb, out, bc, f, fx, hw);
+  if (is_bf16) add_noise_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x0, noise, sa, sb, out, bc, f, fx, hw);
+  else add_noise_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(x0, noise, sa, sb, out, bc, f, fx, hw);
   AAB_LAUNCH_RET();
 }
 
 extern "C" int aab_cast_f32(const float* x, void* y, long n, int is_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (is_bf16) launch_k(cast_f32_kernel<true>, dim3(AAB_GRID(n, 256)), dim3(256), 0, stream, x, y, n);
-  else launch_k(cast_f32_kernel<false>, dim3(AAB_GRID(n, 256)), dim3(256), 0, stream, x, y, n);
+  if (is_bf16) cast_f32_kernel<true><<<dim3(AAB_GRID(n, 256)), dim3(256), 0, stream>>>(x, y, n);
+  else cast_f32_kernel<false><<<dim3(AAB_GRID(n, 256)), dim3(256), 0, stream>>>(x, y, n);
   AAB_LAUNCH_RET();
 }
 
@@ -1055,16 +997,16 @@ extern "C" int aab_video_f32_to_nhwc8(const float* video, long sb, long sc, long
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!video || !out || c < 1 || c > 8 || b < 1 || f < 1 || h < 1 || w < 1) return AAB_ERR_ARG;
   const long total = static_cast<long>(b) * f * h * w;
-  if (is_bf16) launch_k(video_f32_to_nhwc8_kernel<true>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, video, sb, sc, sf, sy, sx, out, b, c, f, h, w);
-  else launch_k(video_f32_to_nhwc8_kernel<false>, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, video, sb, sc, sf, sy, sx, out, b, c, f, h, w);
+  if (is_bf16) video_f32_to_nhwc8_kernel<true><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(video, sb, sc, sf, sy, sx, out, b, c, f, h, w);
+  else video_f32_to_nhwc8_kernel<false><<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(video, sb, sc, sf, sy, sx, out, b, c, f, h, w);
   AAB_LAUNCH_RET();
 }
 
 extern "C" int aab_rgba_finalize_u8(const float* y, int ldc, void* out, long pixels, int is_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!y || !out || ldc < 4 || pixels < 1) return AAB_ERR_ARG;
-  if (is_bf16) launch_k(rgba_finalize_u8_kernel<true>, dim3(AAB_GRID(pixels, 256)), dim3(256), 0, stream, y, ldc, reinterpret_cast<uint8_t*>(out), pixels);
-  else launch_k(rgba_finalize_u8_kernel<false>, dim3(AAB_GRID(pixels, 256)), dim3(256), 0, stream, y, ldc, reinterpret_cast<uint8_t*>(out), pixels);
+  if (is_bf16) rgba_finalize_u8_kernel<true><<<dim3(AAB_GRID(pixels, 256)), dim3(256), 0, stream>>>(y, ldc, reinterpret_cast<uint8_t*>(out), pixels);
+  else rgba_finalize_u8_kernel<false><<<dim3(AAB_GRID(pixels, 256)), dim3(256), 0, stream>>>(y, ldc, reinterpret_cast<uint8_t*>(out), pixels);
   AAB_LAUNCH_RET();
 }
 
@@ -1072,7 +1014,7 @@ extern "C" int aab_pad_cols(const void* src, long lds, void* dst, long rows, int
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!src || !dst || rows < 1 || (cols % 8) || (dst_cols % 8) || (lds % 8) || cols > dst_cols || cols < 8) return AAB_ERR_ARG;
   const long total = rows * (dst_cols / 8);
-  launch_k(pad_cols_kernel, dim3(AAB_GRID(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(src), lds / 8,
+  pad_cols_kernel<<<dim3(AAB_GRID(total, 256)), dim3(256), 0, stream>>>(reinterpret_cast<const uint4*>(src), lds / 8,
            reinterpret_cast<uint4*>(dst), rows, cols / 8, dst_cols / 8);
   AAB_LAUNCH_RET();
 }

@@ -17,10 +17,6 @@
 //   1-tap launches with K <= 640 (ops.pick_two_cta): their main loop is only 5 - 10 k-blocks, so with one CTA the tensor
 //   cores idle through every epilogue; the second CTA's MMAs run under it.  Same control flow, K order and epilogue:
 //   bit-identical to one CTA per SM.
-// * Clusters (IgemmParams::cluster = 2 or 4, 256-column tiles): the CTAs of a cluster take consecutive m-tiles of the same
-//   n-tile; each fetches 1/cluster of the weight tile and multicasts it to all of them, so a k-block reads the weights from
-//   L2 once per cluster instead of once per CTA.  A stage is refilled only after the consumers of every CTA of the cluster
-//   have released it.  Same K order, same epilogue: bit-identical to single CTAs.
 // * Tile widths 32 / 64 / 128 / 160 / 192 / 256: the caller fits the width to N and to the number of tiles per wave, because
 //   a ragged last N tile costs no traffic (TMA zero-fill) but issues every wgmma of its dead columns.
 // * Epilogue: bias / per-sample bias (time embedding) / residual / activation / GEGLU gate, masked at the tile edges, plus
@@ -104,7 +100,6 @@ template <int BN, int MINB, bool GEGLU, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, MINB)
 igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
              const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
-  pdl_trigger();
   using CF = Cfg<BN, MINB>;
   constexpr int STAGES = CF::STAGES;
   constexpr int OUT_BN = GEGLU ? BN / 2 : BN;
@@ -121,14 +116,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int wg = static_cast<int>(threadIdx.x) >> 7;
   const int warp = static_cast<int>(threadIdx.x) >> 5;
   constexpr bool bf16 = BF16;
-  // cluster tiles: CL consecutive m-tiles x one n-tile; this CTA owns m-tile CL * (tile / num_n_tiles) + crank.  With a
-  // number of m-tiles that CL does not divide, the CTAs past the end load m-tile 0 (the cluster moves in lockstep) and
-  // store nothing.
-  const int CL = p.cluster;
-  const int crank = CL > 1 ? static_cast<int>(cluster_ctarank()) : 0;
-  const int tile_first = static_cast<int>(blockIdx.x) / CL;
-  const int tile_step = static_cast<int>(gridDim.x) / CL;
-  const int num_tiles = ((p.num_m_tiles + CL - 1) / CL) * p.num_n_tiles;
+  const int tile_first = static_cast<int>(blockIdx.x);
+  const int tile_step = static_cast<int>(gridDim.x);
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
   const int kb_per_tap = p.kb_per_tap;
   const int k_iters = p.num_taps * kb_per_tap;
 
@@ -138,28 +128,23 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     prefetch_tmap(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], NUM_CONSUMER_WARPS * CL);   // lane 0 of every consumer warp of the cluster releases a stage
+      mbar_init(&empty_bar[i], NUM_CONSUMER_WARPS);   // lane 0 of every consumer warp releases a stage
     }
     fence_barrier_init();
   }
   __syncthreads();
-  if (CL > 1) cluster_sync_all();     // the other CTAs' barriers are initialised before anything is signalled into them
-  pdl_wait();       // everything above (barriers, descriptor prefetch) overlapped the previous kernel's tail
 
   if (wg == 0) {
     // ===================================================== TMA producer
     setmaxnreg_dec<CF::PRODUCER_REGS>();
     if (warp == 0 && elect_one()) {
-      // the weight tile is fetched in NS row slices of BN / NS rows (GEGLU: values and gates are separate slices); CTA crank
-      // of the cluster fetches slices crank, crank + CL, ... and multicasts them
-      const int NS = (CL > 1 || !GEGLU) ? CL : 2;
-      const int slice_rows = BN / (NS > 1 ? NS : 1);
-      const uint16_t mask = static_cast<uint16_t>((1u << CL) - 1u);
+      // the weight tile is fetched in NS row slices of BN / NS rows (GEGLU: values and gates are separate slices)
+      constexpr int NS = GEGLU ? 2 : 1;
+      constexpr int slice_rows = BN / NS;
       uint32_t it = 0;
       for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
         const int nt = tile % p.num_n_tiles;
-        int mt = (tile / p.num_n_tiles) * CL + crank;
-        if (mt >= p.num_m_tiles) mt = 0;
+        int mt = tile / p.num_n_tiles;
         int cb[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -174,7 +159,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           for (int kb = 0; kb < kb_per_tap; ++kb, ++it) {
             const int s = it % STAGES;
             const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait_cluster(&empty_bar[s], ph ^ 1);
+            mbar_wait(&empty_bar[s], ph ^ 1);
             const int kc = kb * BK;
             const int kg = tap * p.Kc + kc;
             mbar_arrive_expect_tx(&full_bar[s], A_STAGE_BYTES + CF::B_STAGE_BYTES);
@@ -184,20 +169,15 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             else
               tma_load_5d(smA + s * A_STAGE_BYTES, &tmA2, &full_bar[s], kc - p.Kc1 + o0, cb[0] + o1, cb[1] + o2,
                           cb[2] + o3, cb[3] + o4);
-            for (int j = crank; j < (NS > 1 ? NS : 1); j += CL) {
+#pragma unroll
+            for (int j = 0; j < NS; ++j) {
               const int t0 = j * slice_rows;                        // first tile row of the slice
               const int row = (GEGLU && t0 >= BN / 2) ? p.N / 2 + n0 + (t0 - BN / 2) : n0 + t0;
-              uint8_t* dst = smB + s * CF::B_STAGE_BYTES + t0 * 128;
-              if (CL > 1) tma_load_3d_mcast(dst, &tmB, &full_bar[s], kg, row, bbatch, mask);
-              else tma_load_3d(dst, &tmB, &full_bar[s], kg, row, bbatch);
+              tma_load_3d(smB + s * CF::B_STAGE_BYTES + t0 * 128, &tmB, &full_bar[s], kg, row, bbatch);
             }
           }
         }
       }
-    }
-    if (CL > 1) {                     // no CTA leaves while a peer may still multicast into it or release its stages
-      __syncwarp();
-      cluster_sync_all();
     }
     return;
   }
@@ -212,15 +192,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const bool scale_acc = (p.flags & AAB_F_SCALE_ACC) != 0;
   const bool stats = !GEGLU && !direct && p.colstats != nullptr;
   uint32_t it = 0;
-
-  auto release = [&](uint32_t stage) {
-    if (lane != 0) return;
-    if (CL > 1) {
-      for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&empty_bar[stage], static_cast<uint32_t>(r));
-    } else {
-      mbar_arrive(&empty_bar[stage]);
-    }
-  };
 
   for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
     float acc[BN / 2];                  // the first wgmma of a tile overwrites it (scale-d = 0)
@@ -239,18 +210,16 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       if (ki > 0) {
         wgmma_wait<1>();
         fence_regs<BN / 2>(acc);
-        release((it - 1) % STAGES);
+        if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       }
     }
     wgmma_wait<0>();
     fence_regs<BN / 2>(acc);
-    release((it - 1) % STAGES);
+    if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
 
     // ---------------- epilogue
     const int nt = tile % p.num_n_tiles;
-    int mt = (tile / p.num_n_tiles) * CL + crank;
-    const bool tile_ok = mt < p.num_m_tiles;                 // a cluster CTA past the last m-tile stores nothing
-    if (!tile_ok) mt = 0;
+    int mt = tile / p.num_n_tiles;
     const int mt_lin = mt;                                  // linear m-tile index (row of the column-statistics table)
     int cb[4];
 #pragma unroll
@@ -272,7 +241,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         rr /= p.box[i];
         v = v && (g[i] < p.dimD[i]);
       }
-      rvalid[h] = v && tile_ok;
+      rvalid[h] = v;
       grow[h] = ((static_cast<long>(g[3]) * p.dimD[2] + g[2]) * p.dimD[1] + g[1]) * p.dimD[0] + g[0];
     }
     const int n0 = nt * OUT_BN;
@@ -417,7 +386,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     if (stats) {
       // the eight warps' partial sums, added in warp order -> one (sum, sumsq) pair per column and m-tile, reproducible
       named_bar_sync(1, 128 * NUM_CONSUMERS);
-      for (int c = static_cast<int>(threadIdx.x) - 128; c < OUT_BN && tile_ok; c += 128 * NUM_CONSUMERS) {
+      for (int c = static_cast<int>(threadIdx.x) - 128; c < OUT_BN; c += 128 * NUM_CONSUMERS) {
         if (n0 + c >= p.n_out) break;
         float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -430,7 +399,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       }
     }
   }
-  if (CL > 1) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -488,64 +456,22 @@ int num_sms() {
 
 template <int BN, int MINB, bool GEGLU, bool BF16>
 static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
-                    int max_ctas, cudaStream_t stream) {
+                    cudaStream_t stream) {
   using CF = Cfg<BN, MINB>;
   static std::atomic<unsigned long long> attr_done{0};
   if (int r = ensure_dyn_smem(igemm_kernel<BN, MINB, GEGLU, BF16>, CF::SMEM_BYTES, attr_done)) return r;
-  const int cl = p.cluster;
-  const int tiles = ((p.num_m_tiles + cl - 1) / cl) * p.num_n_tiles;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = CF::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (cl > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = static_cast<unsigned>(cl);
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
-  int clusters = num_sms() * MINB / cl;     // persistent: MINB CTAs per SM
-  if (cl > 1) {
-    // a cluster's CTAs must fit inside one GPC: ask the driver how many clusters can be resident at once (cached per device)
-    static std::atomic<int> max_clusters[64];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    int mc = max_clusters[dev & 63].load(std::memory_order_acquire);
-    if (mc == 0) {
-      cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
-      int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<BN, MINB, GEGLU, BF16>, &cfg) != cudaSuccess || n < 1) {
-        cudaGetLastError();
-        n = 1;
-      }
-      mc = n;
-      max_clusters[dev & 63].store(mc, std::memory_order_release);
-    }
-    if (clusters > mc) clusters = mc;
-  }
-  if (tiles < clusters) clusters = tiles;
-  if (max_ctas > 0 && clusters > max_ctas / cl) clusters = max_ctas / cl > 0 ? max_ctas / cl : 1;
-  cfg.gridDim = dim3(static_cast<unsigned>(cl * clusters));
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, igemm_kernel<BN, MINB, GEGLU, BF16>, a, a2, b, p);
-  return e == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  int ctas = num_sms() * MINB;     // persistent: MINB CTAs per SM
+  if (tiles < ctas) ctas = tiles;
+  igemm_kernel<BN, MINB, GEGLU, BF16><<<ctas, NUM_THREADS, CF::SMEM_BYTES, stream>>>(a, a2, b, p);
+  return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
 
 template <int BN, bool GEGLU, int MINB = 1>
 static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
-                     int max_ctas, cudaStream_t stream) {
-  if (p.flags & AAB_F_BF16) return launch_t<BN, MINB, GEGLU, true>(a, a2, b, p, max_ctas, stream);
-  return launch_t<BN, MINB, GEGLU, false>(a, a2, b, p, max_ctas, stream);
+                     cudaStream_t stream) {
+  if (p.flags & AAB_F_BF16) return launch_t<BN, MINB, GEGLU, true>(a, a2, b, p, stream);
+  return launch_t<BN, MINB, GEGLU, false>(a, a2, b, p, stream);
 }
 
 }  // namespace aab
@@ -573,6 +499,7 @@ extern "C" int aab_igemm_emits_colstats(const AabIgemmDesc* d) {
 extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!d || !d->a || !d->b || !d->out) return AAB_ERR_ARG;
+  if (d->flags & ~(AAB_F_BF16 | AAB_F_DIRECT | AAB_F_OUT_F32 | AAB_F_GEGLU | AAB_F_SCALE_ACC | AAB_F_TWO_CTA)) return AAB_ERR_ARG;
   const int is_bf16 = (d->flags & AAB_F_BF16) ? 1 : 0;
   const bool geglu = (d->flags & AAB_F_GEGLU) != 0;
   int bn = d->block_n;
@@ -639,29 +566,25 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
       tmA2 = tmA;
     }
   }
-  // clusters sharing each weight tile: 256-column staged tiles with unbatched weights and at least two m-tiles
-  const bool pair = (d->flags & AAB_F_PAIR) != 0 && bn == 256 && !direct && d->b_batch_dim < 0 && p.num_m_tiles >= 2;
-  p.cluster = pair ? (((d->flags & AAB_F_QUAD) && p.num_m_tiles >= 4) ? 4 : 2) : 1;
   {
     long dims[3] = {static_cast<long>(d->num_taps) * d->kc, d->n, d->b_batch > 0 ? d->b_batch : 1};
     long strides[3] = {1, d->ld_b, d->b_batch_stride > 0 ? d->b_batch_stride : static_cast<long>(d->n) * d->ld_b};
-    const int slices = p.cluster > 1 ? p.cluster : (geglu ? 2 : 1);   // rows of one weight-tile slice (see the producer)
-    int box[3] = {BK, bn / slices, 1};
+    int box[3] = {BK, geglu ? bn / 2 : bn, 1};      // one weight-tile slice (GEGLU: values and gates, see the producer)
     int r = make_tmap_16(&tmB, d->b, 3, dims, strides, box, is_bf16, 128);
     if (r) return r;
   }
-  if (two_cta) return launch_bn<64, false, 2>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+  if (two_cta) return launch_bn<64, false, 2>(tmA, tmA2, tmB, p, stream);
   if (geglu) {
-    if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    return launch_bn<256, true>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, p, stream);
+    return launch_bn<256, true>(tmA, tmA2, tmB, p, stream);
   }
   switch (bn) {
-    case 32: return launch_bn<32, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    case 64: return launch_bn<64, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    case 128: return launch_bn<128, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    case 160: return launch_bn<160, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    case 192: return launch_bn<192, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
-    default: return launch_bn<256, false>(tmA, tmA2, tmB, p, d->max_ctas, stream);
+    case 32: return launch_bn<32, false>(tmA, tmA2, tmB, p, stream);
+    case 64: return launch_bn<64, false>(tmA, tmA2, tmB, p, stream);
+    case 128: return launch_bn<128, false>(tmA, tmA2, tmB, p, stream);
+    case 160: return launch_bn<160, false>(tmA, tmA2, tmB, p, stream);
+    case 192: return launch_bn<192, false>(tmA, tmA2, tmB, p, stream);
+    default: return launch_bn<256, false>(tmA, tmA2, tmB, p, stream);
   }
 }
 

@@ -14,8 +14,6 @@
 #define AAB_F_OUT_F32 4   /* output is float32 (direct store only) */
 #define AAB_F_SCALE_ACC 16 /* out = act(acc + bias + bias2) * out_scale + residual (scale BEFORE the residual; direct store only) */
 #define AAB_F_GEGLU 8     /* B rows [0,N/2) are values, [N/2,N) gates: out = value * gelu(gate), N/2 columns */
-#define AAB_F_PAIR 32     /* 256-column staged tiles on clusters of two CTAs sharing each weight tile (TMA multicast) */
-#define AAB_F_QUAD 16384  /* with AAB_F_PAIR: clusters of four (launches with fewer than 4 m-tiles use clusters of two) */
 #define AAB_F_TWO_CTA 64  /* two CTAs per SM (3-stage ring, 80 registers): block_n 64, not GEGLU */
 
 #ifdef __cplusplus
@@ -54,7 +52,6 @@ typedef struct AabIgemmDesc {
   int act;
   int flags;
   int block_n;              // 32 / 64 / 128 / 160 / 192 / 256 (GEGLU: 128 / 256)
-  int max_ctas;             // 0 = one CTA per SM (two with AAB_F_TWO_CTA)
   float* colstats;          // optional [num_m_tiles][n_out][2] fp32: per m-tile column sums (sum, sum of squares) of the ROUNDED
                             // 16-bit outputs over the tile's valid rows -- the statistics of the GroupNorm that follows, taken
                             // where the data already is in registers (staged epilogues only), or NULL
@@ -86,7 +83,6 @@ struct IgemmParams {
   int act;
   int flags;
   float* colstats;
-  int cluster;     /* CTAs per cluster sharing each weight tile: 1, 2 or 4 */
 };
 int make_tmap_16(CUtensorMap* out, const void* base, int rank, const long* dims, const long* strides, const int* box,
                  int is_bf16, int swizzle_bytes = 128);

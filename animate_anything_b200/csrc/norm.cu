@@ -34,8 +34,6 @@ struct GnArgs {
 __global__ void gn_stats_kernel(GnArgs a, double* __restrict__ partial /* [S][chunks][G][2] */,
                                 float* __restrict__ mean_rstd /* [S][G][2] */, unsigned int* __restrict__ ticket /* [S] */,
                                 float eps) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sh[];   // [rpi][C] sums, [rpi][C] squares
   __shared__ bool is_last;
   const int C = a.C1 + a.C2;
@@ -178,8 +176,6 @@ __global__ void gn_stats_kernel(GnArgs a, double* __restrict__ partial /* [S][ch
 
 __global__ void gn_apply_kernel(GnArgs a, const float* __restrict__ mean_rstd, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, int silu, void* __restrict__ y, long ldy) {
-  pdl_trigger();
-  pdl_wait();
   const int C = a.C1 + a.C2;
   const int V = C >> 3;
   const int oct = threadIdx.x % V;
@@ -250,8 +246,6 @@ __global__ void gn_apply_kernel(GnArgs a, const float* __restrict__ mean_rstd, c
 // one.  Two sources = virtual channel concat (channels [0, C1) from cs1, [C1, C1+C2) from cs2).
 __global__ void gn_finalize_kernel(const float* __restrict__ cs1, int C1, const float* __restrict__ cs2, int C2, int tps, long rows,
                                    int groups, float eps, float* __restrict__ mean_rstd) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ double red[2][256];
   const int s = blockIdx.y;
   const int g = blockIdx.x;
@@ -288,94 +282,15 @@ __global__ void gn_finalize_kernel(const float* __restrict__ cs1, int C1, const 
   }
 }
 
-// One warp handles R consecutive rows at a time (all loads of the R rows are issued before any reduction, so that
-// enough bytes are in flight per SM); OPL = 16-byte octets per lane = ceil(C/8/32).  C % 8 == 0, C <= 2048.
-template <int OPL, int R>
-__global__ void __launch_bounds__(256)
-layernorm_kernel(const void* __restrict__ x, long ldx, void* __restrict__ y, long ldy, const float* __restrict__ gamma,
-                 const float* __restrict__ beta, long rows, int C, float eps, int bf16) {
-  pdl_trigger();
-  pdl_wait();
-  const int lane = threadIdx.x & 31;
-  const long warp_global = static_cast<long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const long row0 = warp_global * R;
-  if (row0 >= rows) return;
-  const bool bf = bf16 != 0;
-  const int V = C >> 3;
-  uint4 raw[R][OPL];
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-#pragma unroll
-    for (int i = 0; i < OPL; ++i) {
-      const int o = lane + i * 32;
-      raw[r][i] = make_uint4(0, 0, 0, 0);
-      if (o < V && row0 + r < rows)
-        raw[r][i] = ldg16(reinterpret_cast<const uint8_t*>(x) + ((row0 + r) * ldx + o * 8) * 2);
-    }
-  }
-  const float invc = 1.0f / C;
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    if (row0 + r >= rows) break;
-    float v[OPL][8];
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < OPL; ++i) {
-      const uint32_t w[4] = {raw[r][i].x, raw[r][i].y, raw[r][i].z, raw[r][i].w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = unpack2(w[e], bf);
-        v[i][2 * e] = f.x; v[i][2 * e + 1] = f.y;
-        sum += f.x + f.y;                 // lanes beyond V hold zeros
-      }
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
-    const float mean = sum * invc;
-    float sq = 0.f;
-#pragma unroll
-    for (int i = 0; i < OPL; ++i) {
-      if (lane + i * 32 < V) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; sq += d * d; }
-      }
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, off);
-    const float rstd = rsqrtf(sq * invc + eps);
-#pragma unroll
-    for (int i = 0; i < OPL; ++i) {
-      const int o = lane + i * 32;
-      if (o < V) {
-        const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + o * 8));
-        const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + o * 8) + 1);
-        const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + o * 8));
-        const float4 b1 = __ldg(reinterpret_cast<const float4*>(beta + o * 8) + 1);
-        const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-        uint32_t ow[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          ow[e] = pack2((v[i][2 * e] - mean) * rstd * gg[2 * e] + bb[2 * e],
-                        (v[i][2 * e + 1] - mean) * rstd * gg[2 * e + 1] + bb[2 * e + 1], bf);
-        *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(y) + ((row0 + r) * ldy + o * 8) * 2) =
-            make_uint4(ow[0], ow[1], ow[2], ow[3]);
-      }
-    }
-  }
-}
-
-// LayerNorm v2 (v1 leaves lanes idle for C = 320 / 640): LPR lanes share one row (LPR = 8 / 16 / 32 chosen so that
-// ceil(C/8 / LPR) octets per lane waste no lanes: C=320 -> 8 lanes x 5 octets, 640 -> 16 x 5, 1280 -> 32 x 5), a warp
-// normalises 32/LPR rows at once, persistent warps walk the row groups and the NEXT group's loads are issued before the
-// current group is reduced (register double buffering), so every warp always has loads in flight.  Exact two-pass
-// variance in registers as before; results are per-row (batch-invariant).
+// LayerNorm: LPR lanes share one row (LPR = 8 / 16 / 32 chosen so that ceil(C/8 / LPR) octets per lane waste no lanes:
+// C=320 -> 8 lanes x 5 octets, 640 -> 16 x 5, 1280 -> 32 x 5), a warp normalises 32/LPR rows at once, persistent warps
+// walk the row groups and the NEXT group's loads are issued before the current group is reduced (register double
+// buffering), so every warp always has loads in flight.  Exact two-pass variance in registers; results are per-row
+// (batch-invariant).
 template <int OPL, int LPR>
 __global__ void __launch_bounds__(256)
 layernorm_v2_kernel(const void* __restrict__ x, long ldx, void* __restrict__ y, long ldy, const float* __restrict__ gamma,
                     const float* __restrict__ beta, long rows, int C, float eps, int bf16) {
-  pdl_trigger();
-  pdl_wait();
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPR;
@@ -457,8 +372,6 @@ layernorm_v2_kernel(const void* __restrict__ x, long ldx, void* __restrict__ y, 
 // row softmax: fp32 scores [rows][L] -> 16-bit probabilities (VAE mid-block attention, upcast_softmax semantics)
 __global__ void softmax_rows_kernel(const float* __restrict__ s, long lds, void* __restrict__ p, long ldp, int L, int Lpad,
                                     int bf16) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ float red[32];
   const long row = blockIdx.x;
   const float* sr = s + row * lds;
@@ -516,17 +429,12 @@ static int gn_launch_cfg(int C, long samples, long rows, int* threads, int* rows
 
 // The apply pass is elementwise: its row partition is free (unlike the statistics pass, whose partition fixes the summation
 // order).  The statistics partition can leave a partly filled last wave of CTAs; here the rows are cut so that the launch is
-// ~3 waves of CTAs (AAB_GN_APPLY_WAVES; 0 = the statistics partition), each thread still walking >= 4 rows.
+// ~3 waves of CTAs, each thread still walking >= 4 rows.
 static int gn_apply_rows_per_cta(int C, long samples, long rows, int stats_rpc) {
-  static int waves = -1;
-  if (waves < 0) {
-    const char* e = getenv("AAB_GN_APPLY_WAVES");
-    waves = e ? atoi(e) : 3;
-  }
-  if (waves <= 0) return stats_rpc;
   const int V = C / 8;
   int rpi = 256 / V;
   if (rpi < 1) rpi = 1;
+  const int waves = 3;
   const long slots = 3L * num_sms() * waves;
   long rpc = (rows * samples + slots - 1) / slots;
   if (rpc < 4L * rpi) rpc = 4L * rpi;
@@ -581,12 +489,12 @@ extern "C" int aab_groupnorm(const void* x1, long ld1, int c1, const void* x2, l
   // Two launches rather than one cooperative grid (statistics -> per-sample flag -> apply): a flag wait would serialise the
   // two phases inside every CTA, while two plain launches let the hardware overlap the tail of one with the head of the next.
   dim3 grid(static_cast<unsigned>(chunks), static_cast<unsigned>(samples));
-  launch_k(gn_stats_kernel, dim3(grid), dim3(threads), smem, stream, a, partial, mean_rstd, ticket, eps);
+  gn_stats_kernel<<<dim3(grid), dim3(threads), smem, stream>>>(a, partial, mean_rstd, ticket, eps);
   {
     GnArgs aa = a;
     aa.rows_per_cta = gn_apply_rows_per_cta(C, samples, rows, rpc);
     dim3 ga(static_cast<unsigned>((rows + aa.rows_per_cta - 1) / aa.rows_per_cta), static_cast<unsigned>(samples));
-    launch_k(gn_apply_kernel, dim3(ga), dim3(threads), 0, stream, aa, mean_rstd, gamma, beta, silu, y, ldy);
+    gn_apply_kernel<<<dim3(ga), dim3(threads), 0, stream>>>(aa, mean_rstd, gamma, beta, silu, y, ldy);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
@@ -614,25 +522,16 @@ extern "C" int aab_groupnorm_colstats(const void* x1, long ld1, int c1, const fl
   const int n = tps * (C / groups);
   int fthreads = 32;
   while (fthreads < n && fthreads < 256) fthreads <<= 1;
-  launch_k(gn_finalize_kernel, dim3(static_cast<unsigned>(groups), static_cast<unsigned>(samples)), dim3(fthreads), 0, stream,
+  gn_finalize_kernel<<<dim3(static_cast<unsigned>(groups), static_cast<unsigned>(samples)), dim3(fthreads), 0, stream>>>(
            colstats1, c1, colstats2, c2, tps, rows, groups, eps, mean_rstd);
   dim3 grid(static_cast<unsigned>(chunks), static_cast<unsigned>(samples));
   {
     GnArgs aa = a;
     aa.rows_per_cta = gn_apply_rows_per_cta(C, samples, rows, rpc);
     dim3 ga(static_cast<unsigned>((rows + aa.rows_per_cta - 1) / aa.rows_per_cta), static_cast<unsigned>(samples));
-    launch_k(gn_apply_kernel, dim3(ga), dim3(threads), 0, stream, aa, mean_rstd, gamma, beta, silu, y, ldy);
+    gn_apply_kernel<<<dim3(ga), dim3(threads), 0, stream>>>(aa, mean_rstd, gamma, beta, silu, y, ldy);
   }
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
-}
-
-template <int OPL, int R>
-static void launch_ln(const void* x, long ldx, void* y, long ldy, const float* gamma, const float* beta, long rows, int c,
-                      float eps, int is_bf16, cudaStream_t stream) {
-  const int wpb = 8;
-  const long warps = (rows + R - 1) / R;
-  launch_k(layernorm_kernel<OPL, R>, dim3(static_cast<unsigned>((warps + wpb - 1) / wpb)), dim3(wpb * 32), 0, stream, 
-      x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16);
 }
 
 template <int OPL, int LPR>
@@ -644,7 +543,7 @@ static void launch_ln2(const void* x, long ldx, void* y, long ldy, const float* 
   long ctas = (groups + wpb - 1) / wpb;
   const long cap = 6L * aab::num_sms();                 // persistent: ~6 CTAs of 8 warps per SM
   if (ctas > cap) ctas = cap;
-  launch_k(layernorm_v2_kernel<OPL, LPR>, dim3(static_cast<unsigned>(ctas)), dim3(wpb * 32), 0, stream, x, ldx, y, ldy, gamma, beta, rows, c,
+  layernorm_v2_kernel<OPL, LPR><<<dim3(static_cast<unsigned>(ctas)), dim3(wpb * 32), 0, stream>>>(x, ldx, y, ldy, gamma, beta, rows, c,
                                                                                      eps, is_bf16);
 }
 
@@ -653,29 +552,17 @@ extern "C" int aab_layernorm(const void* x, long ldx, void* y, long ldy, const f
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || (c % 8) || c > 2048 || (ldx % 8) || (ldy % 8)) return AAB_ERR_ARG;
   const int V = c / 8;
-  static int use_v1 = -1;                 // AAB_LN_V1=1: the round-1 kernel (A/B measurements)
-  if (use_v1 < 0) {
-    const char* e = getenv("AAB_LN_V1");
-    use_v1 = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (!use_v1) {
-    // lanes per row: the smallest of 8 / 16 / 32 that keeps <= 8 octets per lane, preferring exact fits
-    if (V <= 8) launch_ln2<1, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 16) launch_ln2<2, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 24) launch_ln2<3, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 32) launch_ln2<4, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 40) launch_ln2<5, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 64) launch_ln2<4, 16>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 80) launch_ln2<5, 16>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 128) launch_ln2<4, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else if (V <= 160) launch_ln2<5, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    else launch_ln2<8, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-    return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
-  }
-  if (V <= 64) launch_ln<2, 4>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-  else if (V <= 96) launch_ln<3, 4>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-  else if (V <= 160) launch_ln<5, 2>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
-  else launch_ln<8, 1>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  // lanes per row: the smallest of 8 / 16 / 32 that keeps <= 8 octets per lane, preferring exact fits
+  if (V <= 8) launch_ln2<1, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 16) launch_ln2<2, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 24) launch_ln2<3, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 32) launch_ln2<4, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 40) launch_ln2<5, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 64) launch_ln2<4, 16>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 80) launch_ln2<5, 16>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 128) launch_ln2<4, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else if (V <= 160) launch_ln2<5, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
+  else launch_ln2<8, 32>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
 
@@ -684,6 +571,6 @@ extern "C" int aab_softmax_rows(const float* s, long lds, void* p, long ldp, lon
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!s || !p || ldp < l) return AAB_ERR_ARG;
   // the probability rows are `ldp` wide: columns l..ldp-1 are written as zeros
-  launch_k(softmax_rows_kernel, dim3(static_cast<unsigned>(rows)), dim3(256), 0, stream, s, lds, p, ldp, l, static_cast<int>(ldp), is_bf16);
+  softmax_rows_kernel<<<dim3(static_cast<unsigned>(rows)), dim3(256), 0, stream>>>(s, lds, p, ldp, l, static_cast<int>(ldp), is_bf16);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }

@@ -4,7 +4,6 @@ to torch compute.
 """
 from __future__ import annotations
 
-import os
 import ctypes as C
 import math
 from typing import Optional, Sequence
@@ -12,23 +11,11 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, F_BF16, F_DIRECT, F_GEGLU, F_OUT_F32, F_PAIR, F_QUAD, F_SCALE_ACC,
-                   F_TWO_CTA, IgemmDesc)
+from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, F_BF16, F_DIRECT, F_GEGLU, F_OUT_F32, F_SCALE_ACC, F_TWO_CTA,
+                   IgemmDesc)
 
 NUM_SMS = 132           # H100 SXM
 IGEMM_PROFILE = None     # bench.py sets this to a list to time every implicit-GEMM launch with CUDA events
-# 256-column tiles on clusters of two CTAs that share each weight tile through TMA multicast.  Off by default: on an H100 SXM
-# at a 400 W power limit the config-2 UNet forward's GEMMs took 264 ms with clusters on the long-K launches against 199 ms
-# on single CTAs (same call, bench.py).  AAB_IGEMM_PAIR=1 enables them where use_pair says, =2 wherever the kernel supports them.
-IGEMM_PAIR = {"0": False, "2": "all"}.get(os.environ.get("AAB_IGEMM_PAIR", "0"), True)
-
-
-def use_pair(k_total: int, n: int) -> bool:
-    """Clusters pay where the main loop dominates and the weight tile is re-read by many m-tiles: long K (>= 960), or
-    K >= 512 with wide outputs; short-K launches are epilogue / latency bound."""
-    if IGEMM_PAIR == "all":
-        return True
-    return bool(IGEMM_PAIR) and (k_total >= 960 or (k_total >= 512 and n >= 1536))
 KERNEL_PROFILE = None    # same for the other kernels: list of {"name", "bytes" (algorithmic HBM bytes), "flops", "ev"}
 
 
@@ -98,11 +85,6 @@ def _tiles_cover_rows_in_order(dim_d, box) -> bool:
     return all(box[j] == 1 for j in range(i, 4))
 
 
-IGEMM_QUAD = os.environ.get("AAB_IGEMM_QUAD", "0") != "0"     # clusters of four instead of two (see igemm.cu)
-GN_COLSTATS = os.environ.get("AAB_GN_COLSTATS", "1") != "0"
-N64_NARROW = os.environ.get("AAB_IGEMM_N64_NARROW", "1") != "0"
-
-
 def pick_block_n(n_out: int, m_tiles: int, geglu: bool = False, k_total: int = 1 << 30) -> int:
     """Widest tile allowed (GEMM columns: 32 / 64 / 128 / 256).  Wide tiles win wherever the main loop dominates: every
     k-block loads the same 16 KiB of activations whatever the width, so a wide tile reads A once for more columns.  A ragged
@@ -112,7 +94,7 @@ def pick_block_n(n_out: int, m_tiles: int, geglu: bool = False, k_total: int = 1
         return 256 if n_out > 64 else 128
     if m_tiles <= 2:
         return 64           # weight-streaming (GEMV-like: text K/V, time embedding): spread the weight rows over many CTAs
-    if n_out <= 64 and N64_NARROW:
+    if n_out <= 64:
         # a 64-column output on a 256-column tile computes and stages mostly zero-filled weight rows; UNet384's 64-channel
         # levels (1-4 M rows) are HBM / latency bound and want the narrow tile.  No shape of the SD UNet / VAE / SVD / CLIP
         # paths has N <= 64.
@@ -161,7 +143,7 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
           out: Optional[torch.Tensor] = None, ld_out: Optional[int] = None, *, bias=None, bias2=None, rows_per_bias2=1,
           residual=None, ld_res=None, act=ACT_NONE, out_scale=1.0, geglu=False, out_f32=False, a2=None, a2_dims=None,
           a2_strides=None, kc1=0, ld_b=None, b_batch=0, b_batch_stride=0, b_batch_dim=-1, block_n=None, direct=False,
-          max_ctas=0, out_rows=None, scale_acc=False, stats=False, ctas_per_sm=None):
+          out_rows=None, scale_acc=False, stats=False, ctas_per_sm=None):
     """Generic launch of the implicit-GEMM kernel. `taps` is a list of 5-int offsets (channel, pix0..pix3).
     `block_n` / `ctas_per_sm` (1, or 2 with `block_n=64`) override the tile width and the CTAs per SM that `pick_two_cta`
     / `pick_block_n` choose from the shape; results are bit-identical whichever runs.
@@ -240,22 +222,16 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         if n_out < 64 and not geglu:
             # 32-column tiles only have the direct-store epilogue; an output that qualifies for the staged epilogue (and
             # its column statistics) takes a 64-column tile whose upper half is a ragged, zero-filled N remainder instead
-            staged_ok = (n_out % 32 == 0 and not out_f32 and not direct and not scale_acc and ld_out % 8 == 0 and
-                         os.environ.get("AAB_IGEMM_N32_DIRECT", "0") == "0")
+            staged_ok = n_out % 32 == 0 and not out_f32 and not direct and not scale_acc and ld_out % 8 == 0
             block_n = 64 if (n_out > 32 or staged_ok) else 32
         else:
             block_n = pick_block_n(n_out, m_tiles, geglu, kc * len(taps))
-    if block_n == 256 and use_pair(kc * len(taps), n):
-        flags |= F_PAIR
-        if IGEMM_QUAD:
-            flags |= F_QUAD
-    elif block_n == 256 and not geglu:
+    if block_n == 256 and not geglu:
         block_n = fit_block_n(n_out, m_tiles, _lib.load().aab_num_sms())
     d.flags = flags
     d.block_n = block_n
-    d.max_ctas = max_ctas
     cstats = None
-    if stats and GN_COLSTATS and not geglu and _tiles_cover_rows_in_order(dim_d, box):
+    if stats and not geglu and _tiles_cover_rows_in_order(dim_d, box):
         d.colstats = 1          # placeholder so that the C-side predicate sees "requested"
         if _lib.load().aab_igemm_emits_colstats(C.byref(d)):
             cstats = torch.empty((m_tiles, n_out, 2), device=a.device, dtype=torch.float32)
@@ -271,7 +247,7 @@ def igemm(a: torch.Tensor, a_dims, a_strides, w: torch.Tensor, n: int, kc: int, 
         _lib.call("aab_igemm", C.byref(d), _stream())
         ev1.record()
         IGEMM_PROFILE.append({"rows": rows, "n": n, "k": kc * len(taps), "taps": len(taps), "block_n": block_n,
-                              "pair": bool(flags & F_PAIR), "two_cta": bool(flags & F_TWO_CTA), "geglu": geglu,
+                              "two_cta": bool(flags & F_TWO_CTA), "geglu": geglu,
                               "residual": residual is not None,
                               "flops": 2.0 * rows * n * kc * len(taps), "ev": (ev0, ev1)})
     else:
@@ -419,8 +395,9 @@ def clip_image_prep(src: torch.Tensor, dtype, out_size: int, patch: int, k_pad: 
     return out
 
 
-def temporal_attn_d64(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
-    bf = _is_bf16(qkv)
+def _temporal_attn(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int,
+                   long_clip: bool):
+    bf = _is_bf16(qkv) | (2 if long_clip else 0)
     out = torch.empty((qkv.shape[0], heads * 64), device=qkv.device, dtype=qkv.dtype)
     rows = qkv.shape[0]
     _profiled("temporal_attn_d64", 2.0 * rows * heads * 64 * 4, 4.0 * b * hw * heads * t * t * 64,
@@ -428,6 +405,10 @@ def temporal_attn_d64(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_
                                 out.stride(0), b, t, hw, heads, 1.0 / math.sqrt(64.0), bf, _stream()),
               shape=(b, t, hw, heads))
     return out
+
+
+def temporal_attn_d64(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
+    return _temporal_attn(qkv, b, t, hw, heads, q_col0, k_col0, v_col0, long_clip=False)
 
 
 # The long-clip kernel keeps a 16-query tile's whole score row (up to 128 keys) in registers; longer clips would need an
@@ -437,14 +418,7 @@ TEMPORAL_MAX_FRAMES = 128
 
 def temporal_attn_long(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
     """`temporal_attn_d64` on the long-clip kernel (bit 1 of `is_bf16`): t in 1..TEMPORAL_MAX_FRAMES, same layout."""
-    bf = _is_bf16(qkv) | 2
-    out = torch.empty((qkv.shape[0], heads * 64), device=qkv.device, dtype=qkv.dtype)
-    rows = qkv.shape[0]
-    _profiled("temporal_attn_d64", 2.0 * rows * heads * 64 * 4, 4.0 * b * hw * heads * t * t * 64,
-              lambda: _lib.call("aab_temporal_attn_d64", _ptr(qkv), qkv.stride(0), q_col0, k_col0, v_col0, _ptr(out),
-                                out.stride(0), b, t, hw, heads, 1.0 / math.sqrt(64.0), bf, _stream()),
-              shape=(b, t, hw, heads))
-    return out
+    return _temporal_attn(qkv, b, t, hw, heads, q_col0, k_col0, v_col0, long_clip=True)
 
 
 def temporal_attn(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0: int, k_col0: int, v_col0: int):
@@ -487,7 +461,7 @@ def groupnorm(x: torch.Tensor, samples: int, rows: int, gamma: torch.Tensor, bet
     ws = _gn_workspace(x.device, need)
     st1 = getattr(x, "_aab_stats", None)
     st2 = None if x2 is None else getattr(x2, "_aab_stats", None)
-    if GN_COLSTATS and st1 is not None and rows % 128 == 0 and (x2 is None or st2 is not None):
+    if st1 is not None and rows % 128 == 0 and (x2 is None or st2 is not None):
         # statistics from the producing GEMMs' epilogues: finalize (tiny) + apply; bytes = one read + one write as before
         assert st1.shape[0] * 128 == x.shape[0] and st1.shape[1] == c1
         _profiled("groupnorm", 2.0 * 2 * x.shape[0] * (c1 + c2), 0.0,

@@ -34,7 +34,7 @@ def _act(x, act):
 
 def _epilogue(acc, bias=None, bias2=None, rows_per_bias2=1, residual=None, act=ACT_NONE, out_scale=1.0, out_f32=False,
               stats=False, **unused):
-    bad = set(unused) - {"block_n", "max_ctas", "direct", "ld_res", "out_rows"}
+    bad = set(unused) - {"block_n", "direct", "ld_res", "out_rows"}
     assert not bad, bad
     if bias is not None:
         acc = acc + bias

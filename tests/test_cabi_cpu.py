@@ -27,6 +27,24 @@ def test_header_compiles_as_c():
                        check=True)
 
 
+def test_igemm_desc_mirror_matches_the_c_struct():
+    """`_lib.IgemmDesc` has the size and field offsets of `AabIgemmDesc` as the C compiler lays it out: a mismatch would
+    have the library read the caller's descriptor at the wrong offsets."""
+    import subprocess
+    import tempfile
+    from animate_anything_b200 import _lib
+    names = [f[0] for f in _lib.IgemmDesc._fields_]
+    prints = "".join(f'printf("%zu\\n", offsetof(AabIgemmDesc, {n}));' for n in names)
+    with tempfile.TemporaryDirectory() as d:
+        c, exe = os.path.join(d, "t.c"), os.path.join(d, "t")
+        open(c, "w").write('#include <stddef.h>\n#include <stdio.h>\n#include "aab200.h"\n'
+                           f'int main(void){{ printf("%zu\\n", sizeof(AabIgemmDesc)); {prints} return 0; }}\n')
+        subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), c, "-o", exe], check=True)
+        got = [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
+    assert got[0] == ctypes.sizeof(_lib.IgemmDesc)
+    assert dict(zip(names, got[1:])) == {n: getattr(_lib.IgemmDesc, n).offset for n in names}
+
+
 def test_library_loads_and_exports_all_symbols():
     from animate_anything_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):

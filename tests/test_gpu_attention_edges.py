@@ -2,9 +2,6 @@
 softmax attention on the same 16-bit inputs."""
 import ctypes as C
 import math
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -12,7 +9,6 @@ import torch
 from util import check
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DTYPES = [torch.float16, torch.bfloat16]
 TOL = {torch.float16: (2e-3, 2e-3), torch.bfloat16: (1.6e-2, 1.6e-2)}
 LOG2E = 1.4426950408889634
@@ -273,38 +269,3 @@ def test_temporal_large_logits(dtype, t, pattern):
     out, ref = _temporal(qkv, b, t, hw, heads)
     check(f"temporal {pattern} t{t} {dtype}", out, ref, *TOL[dtype])
 
-
-_V1_SCRIPT = r"""
-import sys
-import torch
-sys.path.insert(0, sys.argv[1])
-from animate_anything_b200 import ops
-cases = torch.load(sys.argv[2])
-outs = [ops.temporal_attn_d64(c["qkv"].cuda(), *c["args"]).cpu() for c in cases]
-torch.cuda.synchronize()
-torch.save(outs, sys.argv[3])
-"""
-
-
-def test_temporal_v1_matches_v2_bit_for_bit(tmp_path):
-    """The round-1 kernel (AAB_TATTN_V1=1, read once per process: run in a subprocess) and the persistent v2 kernel give
-    identical bits on the same inputs."""
-    from animate_anything_b200 import ops
-    assert os.environ.get("AAB_TATTN_V1", "0") != "1"
-    shapes = [(2, 1, 24, 2), (2, 17, 24, 2), (1, 32, 40, 3), _persistent_shape()]
-    cases, want = [], []
-    for i, (b, t, hw, heads) in enumerate(shapes):
-        for dtype in DTYPES:
-            c = heads * 64
-            qkv = _rand((b * t * hw, 3 * c), dtype, 50 + i, 2.0)
-            args = (b, t, hw, heads, 0, c, 2 * c)
-            want.append(ops.temporal_attn_d64(qkv, *args).cpu())
-            cases.append({"qkv": qkv.cpu(), "args": args})
-    torch.save(cases, tmp_path / "in.pt")
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", _V1_SCRIPT, ROOT, str(tmp_path / "in.pt"),
-                                                                           str(tmp_path / "out.pt")]
-    r = subprocess.run(cmd, env={**os.environ, "AAB_TATTN_V1": "1"}, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = torch.load(tmp_path / "out.pt")
-    for (b, t, hw, heads), g, w in zip([s for s in shapes for _ in DTYPES], got, want):
-        assert torch.equal(g, w), (b, t, hw, heads, g.dtype, int((g != w).sum()))

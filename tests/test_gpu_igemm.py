@@ -176,47 +176,32 @@ def test_batched_gemm_qk():
     check("batched QK^T", out, ref, 1e-3, 1e-3)
 
 
-# ------------------------------------------------------------------------------------------------ clusters sharing the weight tile
-@pytest.fixture(params=["pair", "quad"])
-def pair_mode(request):
-    """pair: clusters of 2; quad: clusters of 4 (each CTA fetches a slice of the weight tile and multicasts it to the others;
-    launches with fewer than 4 m-tiles fall back to clusters of 2 by themselves)."""
-    ops = _ops()
-    old, oldq = ops.IGEMM_PAIR, ops.IGEMM_QUAD
-    ops.IGEMM_PAIR = "all"
-    ops.IGEMM_QUAD = request.param == "quad"
-    yield ops
-    ops.IGEMM_PAIR, ops.IGEMM_QUAD = old, oldq
-
-
+# ------------------------------------------------------------------------------------------------ 256-column tiles
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("residual", [False, True])
 @pytest.mark.parametrize("m,k,n", [(256, 64, 256), (4096, 512, 512), (1000, 640, 1280), (139264 // 8, 320, 320),
                                    (384, 1280, 2560), (130, 320, 256), (8704, 1280, 1280), (640, 320, 576), (896, 2880, 320)])
-def test_pair_linear(pair_mode, dtype, m, k, n):
-    """256-column tiles on clusters: even / odd numbers of m-tiles (130 rows = 2 tiles, 1000 = 8, 384 = 3: the last
-    cluster's CTAs past the end store nothing), ragged last n-tile (320 = 256 + 64), partial last m-tile; bit-identical to the
-    single-CTA kernel (same K order, same epilogue)."""
-    ops = pair_mode
+def test_linear_block_n256(dtype, residual, m, k, n):
+    """256-column tiles (narrowed by `fit_block_n` where N is wider than one tile): even / odd numbers of m-tiles
+    (130 rows = 2 tiles, 1000 = 8, 384 = 3), ragged last n-tile (320 = 256 + 64), partial last m-tile."""
+    ops = _ops()
     x = _rand((m, k), dtype, 1.0, 1)
     w = _rand((n, k), dtype, k ** -0.5, 2)
     b = _rand((n,), torch.float32, 1.0, 3)
-    res = _rand((m, n), dtype, 1.0, 4)
     ref = x.float() @ w.float().t() + b
-    out = ops.linear(x, w, b, block_n=256)
-    check(f"pair linear {m}x{k}x{n} {dtype}", out, ref, *TOL[dtype])
-    out_r = ops.linear(x, w, b, residual=res, block_n=256)
-    check(f"pair linear+res {m}x{k}x{n} {dtype}", out_r, ref + res.float(), *TOL[dtype])
-    ops.IGEMM_PAIR = False
-    single = ops.linear(x, w, b, block_n=256)
-    single_r = ops.linear(x, w, b, residual=res, block_n=256)
-    ops.IGEMM_PAIR = "all"
-    assert torch.equal(out, single) and torch.equal(out_r, single_r)
+    if residual:
+        res = _rand((m, n), dtype, 1.0, 4)
+        out = ops.linear(x, w, b, residual=res, block_n=256)
+        check(f"linear+res bn256 {m}x{k}x{n} {dtype}", out, ref + res.float(), *TOL[dtype])
+    else:
+        out = ops.linear(x, w, b, block_n=256)
+        check(f"linear bn256 {m}x{k}x{n} {dtype}", out, ref, *TOL[dtype])
 
 
-def test_pair_epilogues_conv_and_geglu(pair_mode):
-    ops = pair_mode
-    dtype = torch.bfloat16
-    # GEGLU (values | gates slices fetched by different CTAs of the cluster)
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def test_epilogues_block_n256(dtype):
+    ops = _ops()
+    # GEGLU (values | gates: two slices of the weight tile)
     m, k, n = 1500, 320, 2560
     x = _rand((m, k), dtype, 1.0, 1)
     w = _rand((n, k), dtype, k ** -0.5, 2)
@@ -224,14 +209,14 @@ def test_pair_epilogues_conv_and_geglu(pair_mode):
     y = x.float() @ w.float().t() + b
     ref = y[:, : n // 2] * F.gelu(y[:, n // 2:])
     out = ops.linear(x, w, b, geglu=True)
-    check("pair geglu", out, ref, *TOL[dtype])
+    check("geglu", out, ref, *TOL[dtype])
     # per-sample bias (time embedding) and SiLU epilogues
     n2 = 640
     w2 = _rand((n2, k), dtype, k ** -0.5, 4)
     b2 = _rand((3, n2), torch.float32, 1.0, 5)
     ref2 = x.float() @ w2.float().t() + b2.repeat_interleave(500, dim=0)
-    check("pair bias2", ops.linear(x, w2, None, bias2=b2, rows_per_bias2=500, block_n=256), ref2, *TOL[dtype])
-    check("pair silu", ops.linear(x, w2, None, act=ops.ACT_SILU, block_n=256), F.silu(x.float() @ w2.float().t()), *TOL[dtype])
+    check("bias2", ops.linear(x, w2, None, bias2=b2, rows_per_bias2=500, block_n=256), ref2, *TOL[dtype])
+    check("silu", ops.linear(x, w2, None, act=ops.ACT_SILU, block_n=256), F.silu(x.float() @ w2.float().t()), *TOL[dtype])
     # conv 3x3 with a virtual channel concat (two-source K loop) and an odd number of m-tiles (3 x 24 x 16 px = 9 tiles)
     xa = _rand((3, 24, 16, 128), dtype, 1.0, 6)
     xb = _rand((3, 24, 16, 64), dtype, 1.0, 7)
@@ -239,7 +224,7 @@ def test_pair_epilogues_conv_and_geglu(pair_mode):
     wk = wc.permute(0, 2, 3, 1).reshape(256, -1).contiguous()
     refc = F.conv2d(torch.cat([xa, xb], dim=-1).permute(0, 3, 1, 2).float(), wc.float(), padding=1)
     outc = ops.conv3x3(xa, wk, None, x2=xb, block_n=256)
-    check("pair conv3x3 concat", outc, refc.permute(0, 2, 3, 1).reshape(-1, 256), *TOL[dtype])
+    check("conv3x3 concat", outc, refc.permute(0, 2, 3, 1).reshape(-1, 256), *TOL[dtype])
     # temporal 3-tap conv
     xt = _rand((2 * 5 * 64, 256), dtype, 1.0, 9)
     wt = _rand((256, 3 * 256), dtype, (3 * 256) ** -0.5, 10)
@@ -247,4 +232,4 @@ def test_pair_epilogues_conv_and_geglu(pair_mode):
     x5 = xt.float().reshape(2, 5, 64, 256).permute(0, 3, 1, 2).unsqueeze(-1)           # b c t hw 1
     w5 = wt.float().reshape(256, 3, 256).permute(0, 2, 1).reshape(256, 256, 3, 1, 1)
     reft = F.conv3d(x5, w5, padding=(1, 0, 0)).squeeze(-1).permute(0, 2, 3, 1).reshape(-1, 256)
-    check("pair tconv3", outt, reft, *TOL[dtype])
+    check("tconv3", outt, reft, *TOL[dtype])

@@ -209,7 +209,7 @@ def _producer(ops, x, w, bias, mode, res=None, **kw):
 @pytest.mark.parametrize("mode,m_or_shape,k,n,bn", [("linear", 1024, 320, 320, 64), ("linear", 4352, 640, 640, 128),
                                                      ("linear", 2048, 1280, 1280, 256), ("conv", (3, 32, 32), 320, 320, 128),
                                                      ("conv", (2, 16, 16), 640, 1280, 256)])
-def test_igemm_column_statistics(dtype, mode, m_or_shape, k, n, bn):
+def test_igemm_epilogue_column_statistics(dtype, mode, m_or_shape, k, n, bn):
     """`stats=True`: the epilogue's per-(128-row tile, column) sum / sum of squares of the ROUNDED output it stores."""
     from animate_anything_b200 import ops
     if mode == "linear":
@@ -223,18 +223,12 @@ def test_igemm_column_statistics(dtype, mode, m_or_shape, k, n, bn):
         w = _rand((n, 9 * k), dtype, (9 * k) ** -0.5, 2)
     bias = _rand((n,), torch.float32, 1.0, 3)
     res = _rand((m, n), dtype, 1.0, 4)
-    for pair in ((False, "all") if bn == 256 else (False,)):
-        old = ops.IGEMM_PAIR
-        ops.IGEMM_PAIR = pair
-        try:
-            out = _producer(ops, x, w, bias, mode, res=res, block_n=bn)
-        finally:
-            ops.IGEMM_PAIR = old
-        st = getattr(out, "_aab_stats", None)
-        assert st is not None and tuple(st.shape) == (m // 128, n, 2)
-        o = out.double().reshape(m // 128, 128, n)
-        check(f"colstats sum {mode} {dtype} pair={pair}", st[..., 0], o.sum(1).float(), 1e-5, 1e-3)
-        check(f"colstats sumsq {mode} {dtype} pair={pair}", st[..., 1], (o * o).sum(1).float(), 1e-5, 1e-3)
+    out = _producer(ops, x, w, bias, mode, res=res, block_n=bn)
+    st = getattr(out, "_aab_stats", None)
+    assert st is not None and tuple(st.shape) == (m // 128, n, 2)
+    o = out.double().reshape(m // 128, 128, n)
+    check(f"colstats sum {mode} {dtype}", st[..., 0], o.sum(1).float(), 1e-5, 1e-3)
+    check(f"colstats sumsq {mode} {dtype}", st[..., 1], (o * o).sum(1).float(), 1e-5, 1e-3)
     # an epilogue that cannot emit them (fp32 output) must say so by not attaching anything
     assert getattr(ops.linear(_rand((256, 64), dtype), _rand((64, 64), dtype), None, out_f32=True, stats=True), "_aab_stats", None) is None
 

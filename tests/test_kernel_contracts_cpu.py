@@ -63,18 +63,33 @@ def test_temporal_attn_d64_rejects_bad_arguments_without_a_gpu(buffers):
     assert ta(q_col0=-8) == 1
 
 
+def test_igemm_rejects_undefined_flags_without_a_gpu(buffers):
+    """A flags word with a bit outside the defined AAB_F_* set (32 and 16384 once selected thread-block clusters) returns 1
+    before any CUDA call, instead of launching something other than what the caller asked for."""
+    from animate_anything_b200 import _lib
+    lib, _, p = buffers
+    d = _lib.IgemmDesc()
+    d.a = d.b = d.out = p.value
+    d.kc, d.num_taps, d.n, d.block_n, d.out_scale = 64, 1, 64, 64, 1.0
+    for i in range(4):
+        d.dim_d[i], d.box[i] = (128, 128) if i == 0 else (1, 1)
+    for bit in (32, 16384, 1 << 30):
+        d.flags = bit
+        assert lib.aab_igemm(C.byref(d), None) == 1, bit
+
+
 # ---------------------------------------------------------------------------------------------- coverage table
 # Every entry point of include/aab200.h -> (GPU test that checks it directly, note).  A test id is "file::function"; a row
 # without one says why there is no direct test.  A new entry point without a row fails test_every_entry_point_has_a_row.
 KC = "test_gpu_kernel_contracts.py"
 AE = "test_gpu_attention_edges.py"
 COVERAGE = {
-    "aab_igemm": ("test_gpu_igemm.py::test_linear_plain", "plus conv / tconv / batched / cluster variants in that file"),
-    "aab_igemm_emits_colstats": ("test_gpu_norm_elem.py::test_igemm_column_statistics", ""),
+    "aab_igemm": ("test_gpu_igemm.py::test_linear_plain", "plus conv / tconv / batched / 256-column variants in that file"),
+    "aab_igemm_emits_colstats": ("test_gpu_norm_elem.py::test_igemm_epilogue_column_statistics", ""),
     "aab_flash_attn_d64": (f"{AE}::test_flash_d64_tail_lengths", "plus score patterns, leakage, causal, arguments"),
     "aab_flash_attn_d80": (f"{AE}::test_flash_d80_tail_lengths", "plus test_gpu_clip_vision.py::test_flash_d80_self"),
     "aab_clip_image_prep": ("test_gpu_clip_vision.py::test_clip_image_prep_matches_restatement", ""),
-    "aab_temporal_attn_d64": (f"{AE}::test_temporal_frame_counts", "plus persistent loop, large logits, v1 == v2"),
+    "aab_temporal_attn_d64": (f"{AE}::test_temporal_frame_counts", "plus persistent loop, large logits"),
     "aab_groupnorm_workspace_bytes": ("test_gpu_norm_elem.py::test_groupnorm", "host-side size query, used by every GroupNorm"),
     "aab_groupnorm": ("test_gpu_norm_elem.py::test_groupnorm", ""),
     "aab_groupnorm_colstats": ("test_gpu_norm_elem.py::test_groupnorm_from_producer_statistics", ""),

@@ -1,6 +1,6 @@
 """A/B timing of the HBM-bound kernels at the shapes of a config-2 UNet forward (one CUDA graph of 24 calls over rotating input buffers, replay timed with events: GPU-bound like
-the pipeline's graph replay; a call never finds its own input of the previous iteration in L2).  Variants are selected per PROCESS by the env
-switches read in csrc (AAB_GN_TWO_PASS=1, AAB_LN_V1=1, AAB_TATTN_V1=1); run it twice to compare.
+the pipeline's graph replay; a call never finds its own input of the previous iteration in L2).  To compare two kernel versions, build
+each into its own libaab200.so and run this once per build with AAB_LIB_PATH pointing at it; the library path is printed as the tag.
     python tools/kernel_ab.py [gn|ln|ta|fa|all]      (fa: text cross-attention)
 """
 import os
@@ -10,7 +10,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from animate_anything_b200 import ops  # noqa: E402
+from animate_anything_b200 import _lib, ops  # noqa: E402
 
 what = sys.argv[1] if len(sys.argv) > 1 else "all"
 dt = torch.bfloat16
@@ -45,8 +45,7 @@ def timeit(fn, nbuf, iters=24):
     return e0.elapsed_time(e1) / (3 * iters) * 1e3      # us
 
 
-tag = ",".join(k for k in ("AAB_LN_V1", "AAB_TATTN_V1") if os.environ.get(k) == "1") or "round-2 kernels"
-print(f"variant: {tag}")
+print(f"variant: {_lib.LIB_PATH}")
 print("| kernel | shape | us / call | algorithmic GB/s | frac of 6485.5 |")
 print("|---|---|---|---|---|")
 if what in ("gn", "all"):

@@ -45,7 +45,7 @@ else:
         a["bytes"] += p["bytes"]
         a["flops"] += p["flops"]
     for p in ip:
-        key = ("igemm", f"rows={p['rows']} n={p['n']} k={p['k']} taps={p['taps']} bn={p['block_n']}{'p' if p['pair'] else ''}")
+        key = ("igemm", f"rows={p['rows']} n={p['n']} k={p['k']} taps={p['taps']} bn={p['block_n']}")
         a = agg.setdefault(key, {"n": 0, "ms": 0.0, "bytes": 0.0, "flops": 0.0})
         a["n"] += 1
         a["ms"] += p["ev"][0].elapsed_time(p["ev"][1])
