@@ -13,7 +13,6 @@ is accepted and does not change results.
 """
 from __future__ import annotations
 
-import math
 from typing import Optional, Tuple
 
 import torch
@@ -189,18 +188,9 @@ class AutoencoderKL(ModelBase):
         to_out -> + residual.  One head of dim C: S and O are batched implicit GEMMs, softmax in fp32 (upcast_softmax)."""
         p = ctx.prep.get(attn)
         c = attn.inner_dim
-        n, l = g.n, g.hw
-        lp = (l + 7) // 8 * 8            # K of the P.V GEMM padded with zero probabilities / zero V columns when H*W % 8 != 0
-        hn = ops.groupnorm(x, n, l, p["gn"][0], p["gn"][1], 1e-6, False, 32)
+        hn = ops.groupnorm(x, g.n, g.hw, p["gn"][0], p["gn"][1], 1e-6, False, 32)
         qkv = ops.linear(hn, p["qkv"], p["qkv_b"])                       # [n*l, 3c]
-        q, k = qkv[:, :c], qkv[:, c:2 * c]
-        s = ops.igemm(q, (c, l, n, 1, 1), (1, 3 * c, l * 3 * c, 0, 0), k, l, c, (l, n, 1, 1), (128, 1, 1, 1),
-                      [[0, 0, 0, 0, 0]], ld_b=3 * c, b_batch=n, b_batch_stride=l * 3 * c, b_batch_dim=1, out_f32=True,
-                      out_scale=1.0 / math.sqrt(c))
-        pr = ops.softmax_rows(s, x.dtype, pad_to=lp)                      # [n*l, lp]
-        vt = ops.transpose_batched(qkv, 2 * c, n, l, c, ld=lp)            # [n, c, lp]
-        o = ops.igemm(pr, (lp, l, n, 1, 1), (1, lp, l * lp, 0, 0), vt, c, lp, (l, n, 1, 1), (128, 1, 1, 1),
-                      [[0, 0, 0, 0, 0]], ld_b=lp, b_batch=n, b_batch_stride=c * lp, b_batch_dim=1)
+        o = ops.single_head_attention(qkv, g.n, g.hw, c)
         return ops.linear(o, p["o"][0], p["o"][1], residual=x, out_scale=1.0 / attn.rescale_output_factor, stats=True)
 
     def _mid(self, ctx, mid: UNetMidBlock2D, x, g):

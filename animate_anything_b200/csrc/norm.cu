@@ -402,6 +402,10 @@ __global__ void softmax_rows_kernel(const float* __restrict__ s, long lds, void*
 
 using namespace aab;
 
+// the 16-bit activations move as uint4 and LayerNorm's gamma / beta as float4: a base that is not 16-byte aligned would
+// fault on the GPU, so the entry points reject it
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) % 16) != 0; }
+
 static int gn_launch_cfg(int C, long samples, long rows, int* threads, int* rows_per_cta, int* chunks) {
   if (C % 8) return AAB_ERR_ARG;
   const int V = C / 8;
@@ -465,9 +469,9 @@ extern "C" int aab_groupnorm(const void* x1, long ld1, int c1, const void* x2, l
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int C = c1 + c2;
   if (!x1 || !y || !workspace || groups < 1 || groups > 256 || C % groups || (c1 % 8) || (c2 % 8) || (ld1 % 8) ||
-      (ldy % 8))
+      (ldy % 8) || !gamma || !beta || samples < 1 || rows < 1 || misaligned16(x1) || misaligned16(y))
     return AAB_ERR_ARG;
-  if (c2 > 0 && (!x2 || (ld2 % 8))) return AAB_ERR_ARG;
+  if (c2 > 0 && (!x2 || (ld2 % 8) || misaligned16(x2))) return AAB_ERR_ARG;
   int threads, rpc, chunks;
   int r = gn_launch_cfg(C, samples, rows, &threads, &rpc, &chunks);
   if (r) return r;
@@ -508,9 +512,10 @@ extern "C" int aab_groupnorm_colstats(const void* x1, long ld1, int c1, const fl
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const int C = c1 + c2;
   if (!x1 || !y || !workspace || !colstats1 || groups < 1 || groups > 256 || C % groups || (c1 % 8) || (c2 % 8) || (ld1 % 8) ||
-      (ldy % 8) || (rows % 128) || samples > GN_MAX_SAMPLES)
+      (ldy % 8) || (rows % 128) || samples > GN_MAX_SAMPLES || !gamma || !beta || samples < 1 || rows < 1 ||
+      misaligned16(x1) || misaligned16(y))
     return AAB_ERR_ARG;
-  if (c2 > 0 && (!x2 || !colstats2 || (ld2 % 8))) return AAB_ERR_ARG;
+  if (c2 > 0 && (!x2 || !colstats2 || (ld2 % 8) || misaligned16(x2))) return AAB_ERR_ARG;
   int threads, rpc, chunks;
   int r = gn_launch_cfg(C, samples, rows, &threads, &rpc, &chunks);
   if (r) return r;
@@ -550,7 +555,9 @@ static void launch_ln2(const void* x, long ldx, void* y, long ldy, const float* 
 extern "C" int aab_layernorm(const void* x, long ldx, void* y, long ldy, const float* gamma, const float* beta,
                              long rows, int c, float eps, int is_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!x || !y || (c % 8) || c > 2048 || (ldx % 8) || (ldy % 8)) return AAB_ERR_ARG;
+  if (!x || !y || !gamma || !beta || (c % 8) || c > 2048 || (ldx % 8) || (ldy % 8) || rows < 1 || misaligned16(x) ||
+      misaligned16(y) || misaligned16(gamma) || misaligned16(beta))
+    return AAB_ERR_ARG;
   const int V = c / 8;
   // lanes per row: the smallest of 8 / 16 / 32 that keeps <= 8 octets per lane, preferring exact fits
   if (V <= 8) launch_ln2<1, 8>(x, ldx, y, ldy, gamma, beta, rows, c, eps, is_bf16, stream);
@@ -569,7 +576,7 @@ extern "C" int aab_layernorm(const void* x, long ldx, void* y, long ldy, const f
 extern "C" int aab_softmax_rows(const float* s, long lds, void* p, long ldp, long rows, int l, int is_bf16,
                                 void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!s || !p || ldp < l) return AAB_ERR_ARG;
+  if (!s || !p || rows < 1 || l < 1 || lds < l || ldp < l) return AAB_ERR_ARG;
   // the probability rows are `ldp` wide: columns l..ldp-1 are written as zeros
   softmax_rows_kernel<<<dim3(static_cast<unsigned>(rows)), dim3(256), 0, stream>>>(s, lds, p, ldp, l, static_cast<int>(ldp), is_bf16);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;

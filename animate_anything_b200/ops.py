@@ -365,6 +365,21 @@ def flash_attn_d80(q: torch.Tensor, q_col0: int, kv: torch.Tensor, k_col0: int, 
     return out
 
 
+def single_head_attention(qkv: torch.Tensor, n: int, l: int, c: int) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(c)) V per frame, one head of width c (AutoencoderKL mid-block attention, upcast_softmax).
+    qkv: [n*l, 3c] with columns (q, k, v).  Returns [n*l, c].  S and O are batched implicit GEMMs along the frames, the
+    softmax runs on fp32 scores; the K of the P.V GEMM is l rounded up to a multiple of 8, padded with zero probabilities
+    and zero V columns."""
+    lp = (l + 7) // 8 * 8
+    s = igemm(qkv, (c, l, n, 1, 1), (1, 3 * c, l * 3 * c, 0, 0), qkv[:, c:2 * c], l, c, (l, n, 1, 1), (128, 1, 1, 1),
+              _NO_TAP, ld_b=3 * c, b_batch=n, b_batch_stride=l * 3 * c, b_batch_dim=1, out_f32=True,
+              out_scale=1.0 / math.sqrt(c))
+    pr = softmax_rows(s, qkv.dtype, pad_to=lp)                         # [n*l, lp]
+    vt = transpose_batched(qkv, 2 * c, n, l, c, ld=lp)                 # [n, c, lp]
+    return igemm(pr, (lp, l, n, 1, 1), (1, lp, l * lp, 0, 0), vt, c, lp, (l, n, 1, 1), (128, 1, 1, 1), _NO_TAP, ld_b=lp,
+                 b_batch=n, b_batch_stride=c * lp, b_batch_dim=1)
+
+
 _SRC_TYPES = {torch.uint8: 0, torch.float32: 1, torch.float16: 2, torch.bfloat16: 3}
 
 

@@ -80,22 +80,29 @@ int aab_temporal_attn_d64(const void* qkv, long ld, int q_col0, int k_col0, int 
 /* GroupNorm (+ optional SiLU) over `rows` x (C/groups) per (sample, group); x2 != NULL = virtual channel concat
  * (torch.cat at models/unet_3d_blocks.py:731,828).  Deterministic reductions.  `workspace` must hold
  * aab_groupnorm_workspace_bytes(...) bytes, zero-initialised once (the kernel leaves it reusable).
- * (diffusers ResnetBlock2D.norm1/norm2, TemporalConvLayer GroupNorms, Transformer*.norm, conv_norm_out :514-516). */
+ * (diffusers ResnetBlock2D.norm1/norm2, TemporalConvLayer GroupNorms, Transformer*.norm, conv_norm_out :514-516).
+ * Returns 1 before any launch when: x1, y or workspace is NULL, or x2 when c2 > 0; x1, y or (c2 > 0) x2 is not 16-byte
+ * aligned; gamma or beta is NULL; c1, c2, ld1, ld2 or ldy is not a multiple of 8; groups is outside 1..256 or does not
+ * divide c1 + c2; samples < 1, samples > 4096 or rows < 1. */
 long aab_groupnorm_workspace_bytes(long samples, long rows, int c, int groups);
 int aab_groupnorm(const void* x1, long ld1, int c1, const void* x2, long ld2, int c2, long samples, long rows, int groups,
                   const float* gamma, const float* beta, float eps, int silu, void* y, long ldy, void* workspace,
                   int is_bf16, void* stream);
 /* Same GroupNorm with the statistics pass replaced by the column sums the PRODUCING implicit GEMM wrote (AabIgemmDesc.colstats,
- * [rows_total / 128][c][2] fp32): a tiny finalize kernel + the apply pass.  rows % 128 == 0 (every 128-row tile inside one sample). */
+ * [rows_total / 128][c][2] fp32): a tiny finalize kernel + the apply pass.  rows % 128 == 0 (every 128-row tile inside one sample).
+ * Same rejections as aab_groupnorm, plus a NULL colstats1 (or colstats2 when c2 > 0) and rows % 128 != 0. */
 int aab_groupnorm_colstats(const void* x1, long ld1, int c1, const float* colstats1, const void* x2, long ld2, int c2,
                            const float* colstats2, long samples, long rows, int groups, const float* gamma, const float* beta,
                            float eps, int silu, void* y, long ldy, void* workspace, int is_bf16, void* stream);
 
-/* LayerNorm over C per row (diffusers BasicTransformerBlock.norm1/2/3). */
+/* LayerNorm over C per row (diffusers BasicTransformerBlock.norm1/2/3).  Returns 1 before any launch when: x, y, gamma or
+ * beta is NULL or not 16-byte aligned; c is not a multiple of 8 or above 2048; ldx or ldy is not a multiple of 8; rows < 1. */
 int aab_layernorm(const void* x, long ldx, void* y, long ldy, const float* gamma, const float* beta, long rows, int c,
                   float eps, int is_bf16, void* stream);
 
-/* fp32 scores -> 16-bit probabilities, row softmax (AutoencoderKL mid-block attention, upcast_softmax). */
+/* fp32 scores -> 16-bit probabilities, row softmax (AutoencoderKL mid-block attention, upcast_softmax).  The probability
+ * rows are ldp wide: columns l..ldp-1 are written as +0 (K padding of the following P.V GEMM).  Returns 1 before any launch
+ * when: s or p is NULL; rows < 1; l < 1; lds < l or ldp < l. */
 int aab_softmax_rows(const float* s, long lds, void* p, long ldp, long rows, int l, int is_bf16, void* stream);
 
 /* UNet boundary: frame concat + mask channel + (b f) permute in one pass (models/unet_3d_condition_mask.py:376,424-431)

@@ -355,3 +355,233 @@ def test_cast_f32_special_values(dtype):
     nan = torch.isnan(want)
     assert torch.equal(torch.isnan(y), nan)
     assert torch.equal(y[~nan].view(torch.int16), want[~nan].view(torch.int16))        # bits: signed zeros, infinities
+
+
+# ---------------------------------------------------------------------------------------------- VAE boundary
+def _finite_16bit_values(dtype):
+    """Every finite value of `dtype`, as float32."""
+    bits = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16)
+    v = bits.view(dtype).float()
+    return v[torch.isfinite(v)]
+
+
+def _dec_rows(values, b, f, h, w, ldc, seed):
+    """conv_out-like rows [b*f*h*w, ldc] fp32 carrying `values` (cycled) in channels 0..2; the other channels hold values
+    the kernels must not read."""
+    n = b * f * h * w
+    assert 3 * n >= values.numel()
+    perm = torch.randperm(3 * n, generator=torch.Generator().manual_seed(seed)) % values.numel()
+    y = torch.full((n, ldc), 1e4)
+    y[:, :3] = values[perm].reshape(n, 3)
+    return y.cuda()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("rint", [False, True])
+def test_vae_dec_finalize_u8_every_value(dtype, rint):
+    """Every finite 16-bit value through both roundings, B = 2 and ldc = 5, into the [f, h, b*w, 3] frames.  The kernel
+    depends only on the 16-bit rounding of its input, so this is exhaustive.  The reference is the op sequence of
+    diffusers: tensor2vid `video.mul_(0.5).add_(0.5).clamp_(0, 1)` then numpy `(x * 255).astype("uint8")` (truncation);
+    `postprocess(output_type="pil")`: `(x / 2 + 0.5).clamp(0, 1)`, numpy `(x * 255).round().astype("uint8")`.
+    +-inf, and fp32 inputs of +-1e6 and +-3e38 (+-inf after an fp16 rounding), give 255 and 0: the clamp saturates them."""
+    from animate_anything_b200 import ops
+    import numpy as np
+    b, f, h, w, ldc = 2, 4, 64, 48, 5
+    vals = _finite_16bit_values(dtype)
+    y = _dec_rows(vals, b, f, h, w, ldc, 1)
+    y[:6, 0] = torch.tensor([math.inf, -math.inf, 1e6, -1e6, 3e38, -3e38], device="cuda")
+    out = ops.vae_dec_finalize_u8(y, b, f, h, w, dtype == torch.bfloat16, round_half_even=rint)
+    torch.cuda.synchronize()
+    video = y[:, :3].to(dtype).float().reshape(b, f, h, w, 3).permute(0, 4, 1, 2, 3)          # decode_latents output
+    if rint:
+        x = ((video / 2 + 0.5).clamp(0, 1)).permute(2, 3, 0, 4, 1).reshape(f, h, b * w, 3).cpu().numpy()
+        want = (x * np.float32(255)).round().astype("uint8")
+    else:
+        x = video.mul(0.5).add(0.5).clamp(0, 1).permute(2, 3, 0, 4, 1).reshape(f, h, b * w, 3).cpu().numpy()
+        want = (x * np.float32(255)).astype("uint8")
+    assert x.dtype == np.float32
+    assert torch.equal(out.cpu(), torch.from_numpy(want))
+    # pixel (b=0, f=0, y=0, x=0..5) channel 0: +inf, -inf, and the 16-bit overflows
+    assert out[0, 0, :6, 0].tolist() == [255, 0, 255, 0, 255, 0]
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_vae_dec_finalize_every_value(dtype):
+    """conv_out rows -> float32 video [B, 3, F, H, W]: every finite 16-bit value, plus round-to-nearest-even ties and their
+    fp32 neighbours, rounded once to the model dtype, bit for bit."""
+    from animate_anything_b200 import ops
+    b, f, h, w, ldc = 2, 4, 64, 48, 5
+    vals = torch.cat([_finite_16bit_values(dtype), _ties_and_neighbours(dtype, 2000, 3)])
+    y = _dec_rows(vals, b, f, h, w, ldc, 2)
+    out = ops.vae_dec_finalize(y, b, f, h, w, dtype == torch.bfloat16)
+    torch.cuda.synchronize()
+    want = y[:, :3].to(dtype).float().reshape(b, f, h, w, 3).permute(0, 4, 1, 2, 3)
+    assert torch.equal(out.view(torch.int32), want.contiguous().view(torch.int32))
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_vae_enc_finalize_scaled(dtype):
+    """quant_conv then the 0.18215 latent scale, ldm = 16: the reference rounds the moments to the model dtype and then
+    multiplies the 16-bit tensor (two roundings).  Against float64: within one output ulp plus the half ulp of the
+    intermediate rounding, scaled (and 2^-20 of sum |w m| for the fp32 accumulation).  The double rounding itself:
+    the torch sequence round16(round16(acc) * scale) is matched except where fp32 and float64 accumulation straddle an
+    intermediate rounding boundary, while a single rounding of acc * scale differs for a sizeable share of the outputs."""
+    from animate_anything_b200 import ops
+    b, f, h, w, ldm, scale = 2, 3, 8, 12, 16, 0.18215
+    mom = _randn((b * f * h * w, ldm), dtype, 1, 3.0)
+    wq = torch.randn((8, 8), device="cuda", generator=_gen(2)) * 0.5
+    bq = torch.randn((8,), device="cuda", generator=_gen(3)) * 0.5
+    out = ops.vae_enc_finalize(mom, wq, bq, scale, b, f, h, w)
+    torch.cuda.synchronize()
+
+    def layout(t):
+        return t.reshape(b, f, h, w, 8).permute(0, 4, 1, 2, 3)
+    m = mom[:, :8].double()
+    acc = layout(m @ wq.double().t() + bq.double())
+    mag = layout(m.abs() @ wq.double().abs().t() + bq.double().abs())
+    ref = acc * scale
+    tol = _ulp(ref, dtype) + scale * (_ulp(acc, dtype) / 2 + 2.0 ** -20 * mag)
+    err = (out.double() - ref).abs()
+    assert bool((err <= tol).all()), float((err / tol).max())
+    s32 = float(torch.tensor(scale, dtype=torch.float32))
+    double = (acc.to(dtype).float() * s32).to(dtype)
+    single = (acc * s32).to(dtype)
+    assert (out != double).double().mean().item() <= 0.01
+    assert (double != single).double().mean().item() >= 0.05
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_vae_dec_in(dtype):
+    """latents / 0.18215 rounded to the model dtype (torch's fp32 multiply, bit for bit the same z), post_quant_conv in
+    fp32 (float64 reference: one output ulp plus 2^-20 of sum |w z| + |b|), channels 4..7 exactly +0."""
+    from animate_anything_b200 import ops
+    b, f, h, w = 2, 3, 8, 12
+    lat = _randn((b, 4, f, h, w), dtype, 5, 0.9)
+    wp = torch.randn((4, 4), device="cuda", generator=_gen(6)) * 0.5
+    bp = torch.randn((4,), device="cuda", generator=_gen(7)) * 0.5
+    inv = 1 / 0.18215
+    out = ops.vae_dec_in(lat, inv, wp, bp)
+    torch.cuda.synchronize()
+    assert torch.equal(out[..., 4:].view(torch.int16), torch.zeros_like(out[..., 4:]).view(torch.int16))
+    z = (lat.float() * float(torch.tensor(inv, dtype=torch.float32))).to(dtype).double()
+    z = z.permute(0, 2, 3, 4, 1).reshape(-1, 4)
+    ref = z @ wp.double().t() + bp.double()
+    tol = _ulp(ref, dtype) + 2.0 ** -20 * (z.abs() @ wp.double().abs().t() + bp.double().abs())
+    err = (out.reshape(-1, 8)[:, :4].double() - ref).abs()
+    assert bool((err <= tol).all()), float((err / tol).max())
+
+
+# ---------------------------------------------------------------------------------------------- UNet loop boundary
+def _get_timestep_embedding(t, dim):
+    """diffusers embeddings.get_timestep_embedding(t, dim, flip_sin_to_cos=True, downscale_freq_shift=0), fp32."""
+    half = dim // 2
+    exponent = -math.log(10000) * torch.arange(0, half, dtype=torch.float32, device=t.device) / half
+    emb = t[:, None].float() * torch.exp(exponent)[None, :]
+    emb = torch.cat([torch.sin(emb), torch.cos(emb)], dim=-1)
+    return torch.cat([emb[:, half:], emb[:, :half]], dim=-1)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("dim", [256, 320, 1280])
+def test_timestep_embed(dtype, dim):
+    """t_count in {1, B/2 (CFG: [uncond..., text...]), B}; t = 0, 1, 999 and the SVD noise-level inputs 0.25 * log(sigma).
+    Against diffusers' fp32 embedding: one ulp of the model dtype plus 2^-21 |t * freq|.  Two fp32 evaluations of the
+    argument t * freq differ by up to ~4 of its fp32 roundings (expf is within 2 ulp, and the product rounds once more),
+    and sin / cos pass that on unchanged: at t = 999 that is ~2.4e-4, several fp16 ulps of a small output, so "one ulp"
+    alone holds only for the small t.  float64 sanity bound: one ulp plus 2^-20 (|t * freq| + 1), the same argument error
+    and that of sinf / cosf."""
+    from animate_anything_b200 import ops
+    b = 8
+    vals = [0.0, 1.0, 999.0] + [0.25 * math.log(s) for s in _svd_sigmas()[:-1]]
+    assert len(vals) == b and any(v != int(v) for v in vals)
+    half = dim // 2
+    freq64 = torch.exp(-math.log(10000) * torch.arange(half, dtype=torch.float64, device="cuda") / half)
+    for tc in (1, b // 2, b):
+        for start in range(0, b, tc):
+            t = torch.tensor(vals[start:start + tc], device="cuda", dtype=torch.float32)
+            out = ops.timestep_embed(t, b, dim, dtype)
+            torch.cuda.synchronize()
+            tb = t.repeat(b // tc)                                      # row r takes t[r % t_count]
+            ref32 = _get_timestep_embedding(tb, dim)
+            arg = tb.double()[:, None] * freq64[None]
+            arg2 = torch.cat([arg, arg], -1).abs()
+            err = (out.double() - ref32.double()).abs()
+            tol = _ulp(ref32.double(), dtype) + 2.0 ** -21 * arg2
+            assert bool((err <= tol).all()), (tc, start, float((err / tol).max()))
+            if float(tb.abs().max()) <= 2:
+                assert bool((err <= _ulp(ref32.double(), dtype)).all()), (tc, start)
+            ref64 = torch.cat([torch.cos(arg), torch.sin(arg)], -1)
+            tol = _ulp(ref64, dtype) + 2.0 ** -20 * (arg2 + 1)
+            assert bool(((out.double() - ref64).abs() <= tol).all()), (tc, start)
+
+
+def _coef_rows(kind, steps=10):
+    from animate_anything_b200.schedulers import DDIMScheduler, DPMSolverMultistepScheduler
+    common = dict(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear")
+    if kind == "ddim":
+        s = DDIMScheduler(clip_sample=False, set_alpha_to_one=False, steps_offset=1, **common)
+    else:
+        s = DPMSolverMultistepScheduler(**common)
+    s.set_timesteps(steps)
+    table, hist = s.step_coefficients(s.timesteps)
+    return torch.from_numpy(table).cuda(), hist
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("kind", ["ddim", "dpm"])
+@pytest.mark.parametrize("cfg", [True, False])
+def test_cfg_scheduler_step_coefficients(dtype, kind, cfg):
+    """n = 2 prompts (CFG pairs sample b with b + n), the real DDIM / DPM-Solver++ coefficient tables at step 5, with the
+    x0 history (DPM-Solver++) and without (DDIM passes None).  float64 reference: one output ulp plus 2^-20 of the sum of
+    the magnitudes of the fp32 terms; the history within 2^-20 of its terms."""
+    from animate_anything_b200 import ops
+    n, f, h, w, ldc, g = 2, 3, 6, 5, 16, 7.5
+    t = f + 1
+    nb = 2 * n if cfg else n
+    coef, needs_hist = _coef_rows(kind)
+    assert needs_hist == (kind == "dpm")
+    step = torch.tensor([5], device="cuda", dtype=torch.int32)
+    eps = torch.randn((nb * t * h * w, ldc), device="cuda", generator=_gen(1))
+    eps[:, 4:] = 1e4                                                   # channels the kernel must not read
+    x = _randn((n, 4, f, h, w), dtype, 2, 2.0)
+    hist = torch.randn((n, 4, f, h, w), device="cuda", generator=_gen(3)) if needs_hist else None
+    hist0 = hist.clone() if needs_hist else None
+    out = torch.empty_like(x)
+    ops.cfg_scheduler_step(eps, ldc, cfg, g, x, out, hist, coef, step)
+    torch.cuda.synchronize()
+    e4 = eps.double().reshape(nb, t, h, w, ldc)[..., :4].permute(0, 4, 1, 2, 3)[:, :, 1:]
+    if cfg:
+        e = e4[:n] + g * (e4[n:] - e4[:n])
+        emag = e4[:n].abs() + g * (e4[n:].abs() + e4[:n].abs())
+    else:
+        e, emag = e4, e4.abs()
+    k = coef[5].double()
+    xd = x.double()
+    x0 = k[0] * xd + k[1] * e
+    x0mag = (k[0] * xd).abs() + k[1].abs() * emag
+    ref = k[2] * xd + k[3] * e + k[4] * x0
+    mag = (k[2] * xd).abs() + k[3].abs() * emag + k[4].abs() * x0mag
+    if needs_hist:
+        ref = ref + k[5] * hist0.double()
+        mag = mag + (k[5] * hist0.double()).abs()
+        assert bool(((hist.double() - x0).abs() <= 2.0 ** -20 * x0mag).all())
+    err = (out.double() - ref).abs()
+    tol = _ulp(ref, dtype) + 2.0 ** -20 * mag
+    assert bool((err <= tol).all()), float((err / tol).max())
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_unet_in_assemble_per_sample_masks(dtype):
+    """mask_batch = B with a different mask per sample; sample, cond and mask are non-contiguous views; bit for bit."""
+    from animate_anything_b200 import ops
+    b, f, h, w = 3, 4, 6, 10
+    sample = _randn((b, f, h, w, 4), dtype, 1).permute(0, 4, 1, 2, 3)            # channels-last storage
+    cond = _randn((b, 4, 3, h, w + 2), dtype, 2)[:, :, 1:2, :, 1:1 + w]
+    mask = (_randn((b, 2, 1, h, w), dtype, 3) > 0).to(dtype)[:, 1:]
+    assert not (sample.is_contiguous() or cond.is_contiguous() or mask.is_contiguous())
+    assert not all(torch.equal(mask[0], mask[i]) for i in range(1, b))
+    out = ops.unet_in_assemble(sample, cond, mask, f + 1)
+    torch.cuda.synchronize()
+    ref = torch.cat([mask.expand(b, 1, f + 1, h, w), torch.cat([cond, sample], dim=2)], dim=1).permute(0, 2, 3, 4, 1)
+    assert torch.equal(out[..., :5], ref.contiguous())
+    assert torch.equal(out[..., 5:].view(torch.int16), torch.zeros_like(out[..., 5:]).view(torch.int16))

@@ -1,6 +1,6 @@
-"""CPU: argument checks of the attention entry points (fake buffers, only calls that return before any launch), the table of
-which GPU test covers each C-ABI entry point of include/aab200.h, and the AlphaBlender coefficient the SVD UNet hands to
-`aab_axpby`."""
+"""CPU: argument checks of the attention and normalisation entry points (fake buffers, only calls that return before any
+launch), the table of which GPU test covers each C-ABI entry point of include/aab200.h, and the AlphaBlender coefficient
+the SVD UNet hands to `aab_axpby`."""
 import ctypes as C
 import os
 import re
@@ -63,6 +63,54 @@ def test_temporal_attn_d64_rejects_bad_arguments_without_a_gpu(buffers):
     assert ta(q_col0=-8) == 1
 
 
+def test_groupnorm_rejects_bad_arguments_without_a_gpu(buffers):
+    """Both GroupNorm entry points move the activations in 16-byte pieces: a base that is not 16-byte aligned (a column view
+    at an odd offset) returns 1 instead of faulting; so do missing affine parameters and empty extents."""
+    lib, _, p = buffers
+    mis = C.c_void_p(p.value + 2)
+
+    def gn(x1=p, x2=None, y=p, gamma=p, beta=p, ws=p, c1=64, c2=0, ld1=64, ld2=64, ldy=64, samples=2, rows=256, groups=32):
+        return lib.aab_groupnorm(x1, ld1, c1, x2, ld2, c2, samples, rows, groups, gamma, beta, 1e-5, 1, y, ldy, ws, 0, None)
+
+    def gnc(x1=p, x2=None, y=p, gamma=p, beta=p, ws=p, st2=p, c1=64, c2=0, samples=2, rows=256, groups=32):
+        return lib.aab_groupnorm_colstats(x1, 64, c1, p, x2, 64, c2, st2, samples, rows, groups, gamma, beta, 1e-5, 1, y, 64,
+                                          ws, 0, None)
+    for f in (gn, gnc):
+        assert f(x1=mis) == 1 and f(y=mis) == 1 and f(x2=mis, c2=64) == 1 and f(x2=C.c_void_p(p.value + 8), c2=64) == 1
+        assert f(gamma=None) == 1 and f(beta=None) == 1
+        assert f(samples=0) == 1 and f(samples=-1) == 1 and f(rows=0) == 1 and f(samples=4097) == 1
+        assert f(x1=None) == 1 and f(y=None) == 1 and f(ws=None) == 1 and f(x2=None, c2=64) == 1
+        assert f(groups=0) == 1 and f(groups=3) == 1 and f(groups=512, c1=1024) == 1
+    assert gn(ld1=68) == 1 and gn(ldy=68) == 1 and gn(c1=60) == 1 and gn(x2=p, c2=64, ld2=68) == 1
+    assert gnc(rows=200) == 1 and gnc(x2=p, c2=64, st2=None) == 1                    # 128-row tiles; second statistics
+    assert lib.aab_groupnorm_workspace_bytes(4097, 256, 64, 32) == -1
+    assert lib.aab_groupnorm_workspace_bytes(4096, 256, 64, 32) > 0
+
+
+def test_layernorm_rejects_bad_arguments_without_a_gpu(buffers):
+    """x / y move as uint4 and gamma / beta as float4: each must be 16-byte aligned."""
+    lib, _, p = buffers
+
+    def ln(x=p, y=p, gamma=p, beta=p, ldx=64, ldy=64, rows=4, c=64):
+        return lib.aab_layernorm(x, ldx, y, ldy, gamma, beta, rows, c, 1e-5, 0, None)
+    for off in (2, 4, 8):
+        mis = C.c_void_p(p.value + off)
+        assert ln(x=mis) == 1 and ln(y=mis) == 1 and ln(gamma=mis) == 1 and ln(beta=mis) == 1, off
+    assert ln(gamma=None) == 1 and ln(beta=None) == 1 and ln(x=None) == 1 and ln(y=None) == 1
+    assert ln(rows=0) == 1 and ln(rows=-3) == 1
+    assert ln(c=60) == 1 and ln(c=2056) == 1 and ln(ldx=68) == 1 and ln(ldy=68) == 1
+
+
+def test_softmax_rows_rejects_bad_arguments_without_a_gpu(buffers):
+    lib, _, p = buffers
+
+    def sm(s=p, pr=p, lds=16, ldp=16, rows=4, l=10):
+        return lib.aab_softmax_rows(s, lds, pr, ldp, rows, l, 0, None)
+    assert sm(s=None) == 1 and sm(pr=None) == 1
+    assert sm(rows=0) == 1 and sm(rows=-1) == 1 and sm(l=0) == 1 and sm(l=-5) == 1
+    assert sm(lds=9) == 1 and sm(ldp=9) == 1                            # a score / probability row shorter than l
+
+
 def test_igemm_rejects_undefined_flags_without_a_gpu(buffers):
     """A flags word with a bit outside the defined AAB_F_* set (32 and 16384 once selected thread-block clusters) returns 1
     before any CUDA call, instead of launching something other than what the caller asked for."""
@@ -83,6 +131,7 @@ def test_igemm_rejects_undefined_flags_without_a_gpu(buffers):
 # without one says why there is no direct test.  A new entry point without a row fails test_every_entry_point_has_a_row.
 KC = "test_gpu_kernel_contracts.py"
 AE = "test_gpu_attention_edges.py"
+NC = "test_gpu_norm_contracts.py"
 COVERAGE = {
     "aab_igemm": ("test_gpu_igemm.py::test_linear_plain", "plus conv / tconv / batched / 256-column variants in that file"),
     "aab_igemm_emits_colstats": ("test_gpu_norm_elem.py::test_igemm_epilogue_column_statistics", ""),
@@ -90,14 +139,17 @@ COVERAGE = {
     "aab_flash_attn_d80": (f"{AE}::test_flash_d80_tail_lengths", "plus test_gpu_clip_vision.py::test_flash_d80_self"),
     "aab_clip_image_prep": ("test_gpu_clip_vision.py::test_clip_image_prep_matches_restatement", ""),
     "aab_temporal_attn_d64": (f"{AE}::test_temporal_frame_counts", "plus persistent loop, large logits"),
-    "aab_groupnorm_workspace_bytes": ("test_gpu_norm_elem.py::test_groupnorm", "host-side size query, used by every GroupNorm"),
-    "aab_groupnorm": ("test_gpu_norm_elem.py::test_groupnorm", ""),
-    "aab_groupnorm_colstats": ("test_gpu_norm_elem.py::test_groupnorm_from_producer_statistics", ""),
-    "aab_layernorm": ("test_gpu_norm_elem.py::test_layernorm", ""),
-    "aab_softmax_rows": ("test_gpu_norm_elem.py::test_softmax_rows_and_transpose", ""),
-    "aab_unet_in_assemble": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_groupnorm_workspace_bytes": (f"{NC}::test_groupnorm_workspace_sample_counts",
+                                      "host-side size query, used by every GroupNorm; plus test_groupnorm_chunk_cap"),
+    "aab_groupnorm": (f"{NC}::test_groupnorm_call_sites",
+                      "plus chunk cap, concat split inside a group, strided input, workspace, large mean"),
+    "aab_groupnorm_colstats": (f"{NC}::test_groupnorm_column_statistics", "plus concat split inside a group, large mean"),
+    "aab_layernorm": (f"{NC}::test_layernorm_instances", "plus constant rows, token-0 rows"),
+    "aab_softmax_rows": (f"{NC}::test_softmax_rows_padding_and_patterns", "plus test_vae_mid_attention_chain"),
+    "aab_unet_in_assemble": (f"{KC}::test_unet_in_assemble_per_sample_masks",
+                             "plus test_gpu_norm_elem.py::test_unet_boundary_kernels"),
     "aab_unet_out_finalize": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
-    "aab_timestep_embed": ("test_gpu_norm_elem.py::test_unet_boundary_kernels", ""),
+    "aab_timestep_embed": (f"{KC}::test_timestep_embed", ""),
     "aab_embed_tokens": (f"{KC}::test_embed_tokens", ""),
     "aab_image_to_nhwc16": (f"{KC}::test_image_to_nhwc16", ""),
     "aab_add_rowvec": (f"{KC}::test_add_rowvec", ""),
@@ -112,14 +164,15 @@ COVERAGE = {
     "aab_pad_br": (f"{KC}::test_pad_to_even", ""),
     "aab_copy2d": (f"{KC}::test_copy2d_both_paths", ""),
     "aab_dup_rows": (f"{KC}::test_dup_rows", ""),
-    "aab_transpose": ("test_gpu_norm_elem.py::test_softmax_rows_and_transpose", ""),
-    "aab_cfg_scheduler_step": ("test_gpu_norm_elem.py::test_cfg_scheduler_step", ""),
+    "aab_transpose": ("test_gpu_norm_elem.py::test_softmax_rows_and_transpose", f"plus {NC}::test_vae_mid_attention_chain"),
+    "aab_cfg_scheduler_step": (f"{KC}::test_cfg_scheduler_step_coefficients",
+                               "plus test_gpu_norm_elem.py::test_cfg_scheduler_step"),
     "aab_image_to_nhwc8": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
-    "aab_vae_enc_finalize": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
-    "aab_vae_dec_in": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
-    "aab_vae_dec_finalize": ("test_gpu_norm_elem.py::test_vae_boundary_kernels", ""),
-    "aab_vae_dec_finalize_u8": ("test_gpu_transparent.py::test_masked_latent_to_video_pipeline",
-                                "end to end only: the uint8 frames of the transparent-video pipeline against the reference"),
+    "aab_vae_enc_finalize": (f"{KC}::test_vae_enc_finalize_scaled",
+                             "scale = 1: test_gpu_norm_elem.py::test_vae_boundary_kernels"),
+    "aab_vae_dec_in": (f"{KC}::test_vae_dec_in", ""),
+    "aab_vae_dec_finalize": (f"{KC}::test_vae_dec_finalize_every_value", ""),
+    "aab_vae_dec_finalize_u8": (f"{KC}::test_vae_dec_finalize_u8_every_value", "both roundings, every finite 16-bit value"),
     "aab_add_noise": ("test_gpu_pipeline.py::test_common_ddpm_forward_timesteps_bit_exact", ""),
     "aab_video_f32_to_nhwc8": ("test_gpu_transparent.py::test_video_f32_to_nhwc8_and_rgba_finalize_bit_exact", ""),
     "aab_rgba_finalize_u8": ("test_gpu_transparent.py::test_video_f32_to_nhwc8_and_rgba_finalize_bit_exact", ""),
