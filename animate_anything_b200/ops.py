@@ -447,6 +447,8 @@ def temporal_attn(qkv: torch.Tensor, b: int, t: int, hw: int, heads: int, q_col0
 
 
 # ---------------------------------------------------------------------------------------------- norms
+# Samples (frames, for the spatial norms) per GroupNorm launch: the per-sample tickets of `aab_groupnorm` (csrc/norm.cu)
+GN_MAX_SAMPLES = 4096
 _gn_ws = {}
 
 

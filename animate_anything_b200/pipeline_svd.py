@@ -180,10 +180,11 @@ class StableVideoDiffusionPipeline:
 
     def decode_latents(self, latents, num_frames, decode_chunk_size=14):
         """diffusers StableVideoDiffusionPipeline.decode_latents: [B, F, 4, h, w] -> fp32 [B, 3, F, H, W], decoded in
-        chunks of `decode_chunk_size` frames (the temporal layers of the decoder see one chunk at a time)."""
+        chunks of `decode_chunk_size` frames of the flattened [B * F] axis (the temporal layers of the decoder see one chunk
+        at a time; when the chunk size does not divide F, a chunk holds the last frames of one video and the first of the
+        next, and they mix in those layers, as in diffusers)."""
+        b = latents.shape[0]
         lat = latents.flatten(0, 1)
-        if latents.shape[0] != 1:
-            raise NotImplementedError("one video per call (as the reference's mask handling implies, models/pipeline.py:372)")
         outs = []
         inv = 1.0 / self.vae.config.scaling_factor
         for i in range(0, lat.shape[0], decode_chunk_size):
@@ -192,7 +193,8 @@ class StableVideoDiffusionPipeline:
             # scale of a [n, 4, h, w] latent, once per clip)
             z = (z * inv).contiguous()
             outs.append(self.vae.decode_chunk_video(z, z.shape[0]))           # [1, 3, n, H, W] fp32
-        return torch.cat(outs, dim=2)                                         # [1, 3, F, H, W]: chunks are consecutive frames
+        video = torch.cat(outs, dim=2)                                        # [1, 3, B*F, H, W]: chunks are consecutive frames
+        return video.view(3, b, num_frames, *video.shape[-2:]).transpose(0, 1)    # [B, 3, F, H, W]
 
     def _output_frames(self, latents, num_frames, decode_chunk_size, output_type):
         """diffusers svd_tensor2vid(decode_latents(...), image_processor, output_type) -> one list / array / tensor of
@@ -206,8 +208,6 @@ class StableVideoDiffusionPipeline:
             return [self.image_processor.postprocess(frames[b].permute(1, 0, 2, 3), output_type)
                     for b in range(frames.shape[0])]                          # diffusers svd tensor2vid
         import PIL.Image
-        if latents.shape[0] != 1:
-            raise NotImplementedError("one video per call (as the reference's mask handling implies, models/pipeline.py:372)")
         lat = latents.flatten(0, 1)
         inv = 1.0 / self.vae.config.scaling_factor
         images = []
@@ -215,7 +215,42 @@ class StableVideoDiffusionPipeline:
             z = (lat[i: i + decode_chunk_size] * inv).contiguous()          # as decode_latents
             u8 = self.vae.decode_chunk_frames_u8(z, z.shape[0]).cpu().numpy()   # [n, H, W, 3]
             images.extend(PIL.Image.fromarray(im) for im in u8)
-        return [images]
+        return [images[i: i + num_frames] for i in range(0, len(images), num_frames)]     # one list of frames per video
+
+    def _check_text_batch_call(self, batch_size, num_frames, height, width, cfg, num_videos_per_prompt, generator, mask,
+                               condition_latent, latents):
+        """`TextStableVideoDiffusionPipeline.__call__` with B images: the errors the reference raises later (or a limit of the
+        kernels), raised before the first launch.  On the base class because the reference calls the Text `__call__` unbound
+        on a stock pipeline (app_svd.py:120)."""
+        if num_videos_per_prompt != 1:
+            # the reference repeats the embeddings and latents but not the mask / condition_latent, and its
+            # torch.cat([mask, latent_model_input, condition_latent], dim=2) (:688) fails
+            raise NotImplementedError("num_videos_per_prompt > 1 is not supported: pass the image several times instead")
+        if isinstance(generator, list):
+            raise TypeError("randn() received a list of generators; one torch.Generator seeds the whole image batch")
+        lat = (height // self.vae_scale_factor, width // self.vae_scale_factor)
+        motion_mask = self.unet.config.in_channels == 9
+        if cfg and mask is None:
+            raise TypeError("expected Tensor as element 0 in argument 0, but got NoneType (torch.cat([mask] * 2), "
+                            "models/pipeline.py:609)")
+        if motion_mask:
+            if mask is None:
+                raise TypeError("a 9-channel UNet needs `mask` [B, F, 1, h, w] (models/pipeline.py:688)")
+            if tuple(mask.shape) != (batch_size, num_frames, 1) + lat:
+                raise RuntimeError(f"Sizes of tensors must match except in dimension 2: mask {tuple(mask.shape)} vs latents "
+                                   f"{(batch_size, num_frames, 4) + lat} (models/pipeline.py:688)")
+        if condition_latent is not None and tuple(condition_latent.shape) != (batch_size, num_frames, 4) + lat:
+            raise RuntimeError(f"Sizes of tensors must match except in dimension 2: condition_latent "
+                               f"{tuple(condition_latent.shape)} vs latents {(batch_size, num_frames, 4) + lat} "
+                               f"(models/pipeline.py:688-690)")
+        want = (batch_size, num_frames, self.unet.config.in_channels // 2) + lat
+        if latents is not None and tuple(latents.shape) != want:
+            raise RuntimeError(f"Sizes of tensors must match except in dimension 2: latents {tuple(latents.shape)} vs "
+                               f"{want} (models/pipeline.py:688-690)")
+        unet_frames = (2 if cfg else 1) * batch_size * num_frames
+        if unet_frames > ops.GN_MAX_SAMPLES:
+            raise ValueError(f"the UNet batch holds {unet_frames} frames ((2 under guidance) x {batch_size} videos x "
+                             f"{num_frames} frames); its GroupNorm kernel takes at most {ops.GN_MAX_SAMPLES}")
 
     @torch.no_grad()
     def __call__(self, image, height: int = 576, width: int = 1024, num_frames: Optional[int] = None,
@@ -386,7 +421,11 @@ class TextStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
     halves (:602-604); 9-channel UNets get cat([mask, x, cond]), 8-channel ones cat([x, cond]) (:657-660).
     The call the reference makes (app_svd.py:120-133) is condition_type="image" with `condition_latent` and a per-frame mask.  A
     multi-token context ("text" / both) is passed to the UNet as the reference does -- and fails there exactly as it does under
-    the pinned diffusers 0.24, whose temporal transformer broadcasts the context with a literal 1 token (RuntimeError)."""
+    the pinned diffusers 0.24, whose temporal transformer broadcasts the context with a literal 1 token (RuntimeError).
+
+    Several images make several videos in one call (`batch_size = len(image)`, :583-588): the CLIP tower and the VAE encode take
+    the whole image batch, the UNet runs at batch 2B under guidance, and `decode_latents` decodes the flattened [B * F] frames in
+    chunks of `decode_chunk_size`, so a chunk that does not divide F holds frames of two videos (see `decode_latents`)."""
 
     @torch.no_grad()
     def __call__(self, image, prompt_embeds=None, negative_prompt_embeds=None, height: int = 576, width: int = 1024,
@@ -409,8 +448,8 @@ class TextStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
         cfg = max_guidance_scale > 1.0
         image_t = self.image_processor.preprocess(image, height=height, width=width).to(device)
         batch_size = image_t.shape[0]
-        if batch_size * num_videos_per_prompt != 1:
-            raise NotImplementedError("one video per call on the sm_90a path")
+        self._check_text_batch_call(batch_size, num_frames, height, width, cfg, num_videos_per_prompt, generator, mask,
+                                    condition_latent, latents)
 
         def _text():
             if prompt_embeds is None or (cfg and negative_prompt_embeds is None):
@@ -431,16 +470,13 @@ class TextStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
         else:
             emb = torch.cat([_img(), _text()], dim=1)
         motion_mask = self.unet.config.in_channels == 9
-        if cfg and mask is None:
-            raise TypeError("expected Tensor as element 0 in argument 0, but got NoneType (torch.cat([mask] * 2), "
-                            "models/pipeline.py:590)")
         fps = fps - 1
         noise = torch.randn(image_t.shape, generator=generator, device=generator.device if generator is not None else device,
                             dtype=image_t.dtype).to(device)
         image_t = image_t + noise_aug_strength * noise
         lat_h, lat_w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if condition_latent is None:
-            il = self.vae.encode(image_t.to(dtype)).latent_dist.mode().to(dtype).contiguous()          # [1, 4, h, w]
+            il = self.vae.encode(image_t.to(dtype)).latent_dist.mode().to(dtype).contiguous()          # [B, 4, h, w]
             cond = il.reshape(1, batch_size, 1, 4, lat_h, lat_w)
             zero_uncond = True
         else:
@@ -463,11 +499,6 @@ class TextStableVideoDiffusionPipeline(StableVideoDiffusionPipeline):
         gs_f32 = gs[0].float().contiguous()
         m16 = None
         if motion_mask:
-            if mask is None:
-                raise TypeError("a 9-channel UNet needs `mask` [B, F, 1, h, w] (models/pipeline.py:657)")
-            if tuple(mask.shape) != (batch_size, num_frames, 1, lat_h, lat_w):
-                raise RuntimeError(f"Sizes of tensors must match except in dimension 2: mask {tuple(mask.shape)} vs latents "
-                                   f"{(batch_size, num_frames, 4, lat_h, lat_w)} (models/pipeline.py:657)")
             m16 = mask.to(device=device, dtype=dtype).reshape(batch_size, num_frames, lat_h, lat_w).contiguous()
         in_ch = self.unet.config.in_channels
         b_unet = (2 if cfg else 1) * batch_size
