@@ -273,6 +273,18 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               cp_async_16(srow0 + (s & 1) * SLAB_BYTES + h * H_OFF + vec_off, resrow(h) + (n0 + s * SLAB_COLS + 8 * q) * 2);
           cp_async_commit();
         };
+        // bias of slab s (GEGLU: value and gate columns) in registers one slab ahead: a load issued where it is added would
+        // put an L2 round trip on the conversion path of every slab
+        float2 bval[2][SLAB_COLS / 8], bgate[2][SLAB_COLS / 8];
+        auto fetch_bias = [&](int s) {
+#pragma unroll
+          for (int j = 0; j < SLAB_COLS / 8; ++j) {
+            const int col = n0 + s * SLAB_COLS + j * 8 + 2 * q;
+            bval[s & 1][j] = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+            if (GEGLU) bgate[s & 1][j] = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
+          }
+        };
+        if (p.bias != nullptr && nslab > 0) fetch_bias(0);
         __syncwarp();                                          // the previous tile's last slab has been read
         if (has_res) fetch_res(0);
 #pragma unroll
@@ -282,6 +294,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           if (has_res) cp_async_wait<0>();
           __syncwarp();                                        // this slab's residual has landed; the other buffer has been read
           if (has_res && s + 1 < nslab) fetch_res(s + 1);      // in flight while this slab is converted
+          if (p.bias != nullptr && s + 1 < nslab) fetch_bias(s + 1);
 #pragma unroll
           for (int j = 0; j < SLAB_COLS / 8; ++j) {
             const int jj = s * (SLAB_COLS / 8) + j;
@@ -296,15 +309,15 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               if (GEGLU) {
                 float g[2] = {acc[4 * (jj + BN / 16) + 2 * h], acc[4 * (jj + BN / 16) + 2 * h + 1]};
                 if (p.bias != nullptr) {
-                  const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-                  const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
+                  const float2 bv = bval[s & 1][j];
+                  const float2 bg = bgate[s & 1][j];
                   x[0] += bv.x; x[1] += bv.y;
                   g[0] += bg.x; g[1] += bg.y;
                 }
                 *wp = pack2(x[0] * gelu_fast_f(g[0]), x[1] * gelu_fast_f(g[1]), bf16);
               } else {
                 if (p.bias != nullptr) {
-                  const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                  const float2 b = bval[s & 1][j];
                   x[0] += b.x; x[1] += b.y;
                 }
                 if (has_bias2 && rvalid[h]) {
