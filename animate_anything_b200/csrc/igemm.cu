@@ -8,22 +8,24 @@
 //   shifted pixel coordinate; out-of-bounds pixels are zero-filled by the TMA unit (= conv zero padding).
 // * B (weights, [N, K] K-contiguous) is TMA-loaded; both land in shared memory in the 128B-swizzled K-major layout
 //   that wgmma reads through matrix descriptors.  A stage ring of mbarrier-guarded buffers feeds the tensor cores.
-// * Warp specialisation: warpgroup 0 is the TMA producer (one elected thread), warpgroups 1 and 2 each own 64 rows of
-//   the 128 x BN tile and keep their accumulators in registers (m64nBNk16 wgmma, fp32).
+// * Warp specialisation: warp 0 of warpgroup 0 is the TMA producer (one elected thread), warps 1 - 3 of warpgroup 0 are
+//   the epilogue warps, warpgroups 1 and 2 each own 64 rows of the 128 x BN tile and keep their accumulators in registers
+//   (m64nBNk16 wgmma, fp32).
 // * Persistent CTAs (one per SM) walk the tile list n-fastest so that the CTAs running concurrently share the same
 //   A rows (L2 hits) while the weights stay L2-resident; the producer runs ahead into the next tile while the
 //   consumers finish the epilogue of the current one.
 // * Two CTAs per SM (AAB_F_TWO_CTA, template MINB = 2, 64-column tiles, 3-stage ring, 80 registers per thread) for the
 //   1-tap launches with K <= 640 (ops.pick_two_cta): their main loop is only 5 - 10 k-blocks, so with one CTA the tensor
-//   cores idle through every epilogue; the second CTA's MMAs run under it.  Same control flow, K order and epilogue:
+//   cores idle through every ring refill; the second CTA's MMAs run under it.  Same control flow, K order and epilogue:
 //   bit-identical to one CTA per SM.
 // * Tile widths 32 / 64 / 128 / 160 / 192 / 256: the caller fits the width to N and to the number of tiles per wave, because
 //   a ragged last N tile costs no traffic (TMA zero-fill) but issues every wgmma of its dead columns.
-// * Epilogue: bias / per-sample bias (time embedding) / residual / activation / GEGLU gate, masked at the tile edges, plus
-//   optional per-tile column statistics for the GroupNorm that follows.  16-bit outputs are transposed through a per-warp
-//   shared-memory slab so that the residual comes in and the result leaves as 16-byte accesses of whole 64-byte row
-//   segments (the accumulator layout alone gives 4-byte accesses, half a sector per row); the stores are not waited for, so
-//   they drain under the next tile's main loop.  fp32 / odd-N / scaled outputs are stored per element from the registers.
+// * Staged epilogue (16-bit outputs TMA can address): the consumers add bias / per-sample bias (time embedding) / residual,
+//   apply SiLU or the GEGLU gate and round, writing in place over the residual in a 128 x OUT_BN shared-memory staging tile,
+//   and go straight back to the main loop of their next tile.  The producer thread loads the residual into the staging tile
+//   by TMA; the epilogue warps stage the tile's bias rows in shared memory, take the per-tile column statistics for the
+//   GroupNorm that follows from the staged 16-bit values, and store the tile by TMA.  fp32 / odd-N / scaled outputs are
+//   stored per element from the registers (direct epilogue).
 //
 // Replaces, for the reference path (SURVEY.md section 8a): cuDNN conv2d/conv3d and cuBLAS linear calls made by
 // diffusers ResnetBlock2D / TemporalConvLayer / Transformer2DModel / TransformerTemporalModel / AutoencoderKL
@@ -39,35 +41,42 @@ constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;       // 16 KiB
 constexpr int NUM_CONSUMERS = 2;                 // consumer warpgroups, 64 tile rows each
 constexpr int NUM_THREADS = 128 * (1 + NUM_CONSUMERS);
-constexpr int NUM_CONSUMER_WARPS = 4 * NUM_CONSUMERS;
+constexpr int NUM_CONSUMER_THREADS = 128 * NUM_CONSUMERS;
+constexpr int NUM_EPI_THREADS = 96;              // warps 1 - 3 of warpgroup 0: column statistics and the output store
 
-// staged epilogue: every consumer warp owns two slabs (used in turn) of its 16 tile rows x 32 columns: 64-byte rows, 16-byte
-// chunks XOR-swizzled by the row pair so that neither the accumulator-layout word accesses nor the 16-byte row accesses
-// conflict on a bank
-constexpr int SLAB_COLS = 32;
-constexpr int SLAB_BYTES = 16 * SLAB_COLS * 2;   // 1 KiB
+// staged epilogue: the 128 x OUT_BN 16-bit output tile sits in shared memory as OUT_BN / 32 sub-tiles of 128 rows x 64 bytes
+// in the TMA SWIZZLE_64B layout (16-byte chunk c of row r at chunk c ^ ((r >> 1) & 3)): one TMA box each way, and a warp's
+// accumulator-layout 4-byte accesses (8 rows x 4 words of one chunk) fall on 32 distinct banks
+constexpr int SUB_COLS = 32;
+constexpr int SUB_BYTES = BM * SUB_COLS * 2;     // 8 KiB
 
-// Shared-memory ring and register split per tile width and CTAs per SM (MINB).
-//   MINB = 1: 160 - 200 KiB of operands in flight whatever BN, plus the column-statistics scratch and the epilogue slabs,
-//             inside the 227 KiB a block may use; the producer warpgroup gives registers to the consumers (40 / 232).
+// Shared-memory ring and register split per tile width, CTAs per SM (MINB) and GEGLU (half as many output columns).
+//   MINB = 1: the ring, the output staging tile (128 x OUT_BN x 2 bytes) and the tile's bias rows inside the 227 KiB a block
+//             may use; the producer warpgroup gives registers to the consumers (56 / 224: the epilogue warps spill below 56).
+//             BN 256 keeps 3 stages (212.3 KiB), BN 192 4 (211.5), BN 160 5 (223.1), BN 128 6 (226.8), BN 64 8 (210),
+//             GEGLU 256 4 (226.8), GEGLU 128 6 (210).
 //   MINB = 2: the short-K 1-tap launches (ops.pick_two_cta), 64-column tiles only: two CTAs per SM, so that one CTA's
-//             epilogue and ring refill run under the other's MMAs.  Shared memory: a CTA gets at most 113 KiB (half of the SM's
-//             228 KiB less the 1 KiB reserved per CTA); 3 stages = 72 KiB of operands + 4 KiB statistics + 16 KiB slabs +
-//             pad = 93.25 KiB (a fourth stage would need 117.25).  Registers: __launch_bounds__(384, 2) caps every thread at
-//             80 (2 x 384 x 80 <= 64 K), 30 720 per CTA = producer 32 + consumers 104.  The compiler allocates the consumer
+//             main loop runs while the other waits for its ring refill.  Shared memory: a CTA gets at most 113 KiB (half of
+//             the SM's 228 KiB less the 1 KiB reserved per CTA); 3 stages = 72 KiB of operands + 16 KiB staging tile + bias +
+//             pad = 90 KiB (a fourth stage would need 114).  Registers: __launch_bounds__(384, 2) caps every thread at
+//             80 (2 x 384 x 80 <= 64 K), 30 720 per CTA >= producer 56 + consumers 88.  The compiler allocates the consumer
 //             code within the 80 of the launch bounds: the 32 accumulators of BN = 64 fit with no spill, the 64 of
-//             BN = 128 (and so GEGLU) do not compile.  A producer below 32 spills its tile / tap coordinates.
-template <int BN, int MINB = 1>
+//             BN = 128 (and so GEGLU) do not compile.  The producer and epilogue warps spill below 56.
+template <int BN, int MINB = 1, bool GEGLU = false>
 struct Cfg {
-  static_assert(MINB == 1 || (MINB == 2 && BN == 64), "two CTAs per SM are instantiated at BN = 64 only");
-  static constexpr int STAGES = (MINB == 2) ? 3 : (BN >= 192) ? 4 : (BN == 160) ? 5 : (BN == 128) ? 6 : 8;
-  static constexpr int PRODUCER_REGS = (MINB == 2) ? 32 : 40;
-  static constexpr int CONSUMER_REGS = (MINB == 2) ? 104 : 232;
+  static_assert(MINB == 1 || (MINB == 2 && BN == 64 && !GEGLU), "two CTAs per SM are instantiated at BN = 64 only");
+  static constexpr int OUT_BN = GEGLU ? BN / 2 : BN;
+  static constexpr int STAGES = (MINB == 2) ? 3 : (BN == 256) ? (GEGLU ? 4 : 3) : (BN == 192) ? 4 : (BN == 160) ? 5
+                                : (BN == 128) ? 6 : 8;
+  static constexpr int PRODUCER_REGS = 56;
+  static constexpr int CONSUMER_REGS = (MINB == 2) ? 88 : 224;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
-  static constexpr int STATS_BYTES = NUM_CONSUMER_WARPS * BN * 2 * 4;   // per-warp (sum, sum of squares) per column
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + STATS_BYTES +
-                                    NUM_CONSUMER_WARPS * 2 * SLAB_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int OUT_BYTES = BM * OUT_BN * 2;
+  static constexpr int BIAS_FLOATS = 3 * OUT_BN;   // bias | per-sample bias of the tile's first and last sample (GEGLU: bias of values | gates)
+  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + OUT_BYTES + BIAS_FLOATS * 4 +
+                                    1024 /*align*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= (MINB == 2 ? 113 : 227) * 1024, "tile configuration exceeds the shared memory of an SM");
+  static_assert(B_STAGE_BYTES % 1024 == 0, "the staging tile must stay 1024-byte aligned for its swizzle");
   static_assert(128 * PRODUCER_REGS + 128 * NUM_CONSUMERS * CONSUMER_REGS <= NUM_THREADS * (MINB == 2 ? 80 : 168),
                 "setmaxnreg split exceeds the registers the launch bounds give a CTA");
 };
@@ -90,28 +99,52 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_addr, uint32_t
   }
 }
 
+// byte offset of the 4-byte word (row r, column pair cp) in the staging tile
+__device__ __forceinline__ int stage_word_off(int r, int cp) {
+  return (cp >> 4) * SUB_BYTES + r * (SUB_COLS * 2) + ((((cp >> 2) & 3) ^ ((r >> 1) & 3)) << 4) + (cp & 3) * 4;
+}
+
 // GEGLU: B tile = [values | gates] (BN/2 rows each), out = value * gelu(gate), BN/2 columns.
 // Epilogue flavours (runtime, uniform per launch):
-//   staged  (no AAB_F_DIRECT): n_out % 32 == 0, 16-bit output, 16-byte aligned rows, at most one of residual / per-sample
-//                              bias / SiLU, no scaling; goes through the warp's shared-memory slab and leaves as 16-byte
-//                              stores of whole 64-byte row segments; may emit column statistics
+//   staged  (no AAB_F_DIRECT): n_out % 32 == 0, 16-bit output, rows TMA can address, at most one of residual / per-sample
+//                              bias / SiLU, no scaling; the consumers convert into the shared-memory staging tile and go
+//                              back to their main loop, warps 1 - 3 take the column statistics and store the tile by TMA;
+//                              the residual comes in by TMA
 //   direct  (AAB_F_DIRECT):    any n_out, fp32 or 16-bit output, every flag combination, masked per element
+//
+// Staged epilogue barriers, one phase per tile of the CTA (j = the CTA's tile count so far, parity j & 1):
+//   free  (96 arrivals):       the epilogue warps have read tile j's staging tile and its TMA store has read it too.  The
+//                              producer waits for phase j - 1 (parity (j & 1) ^ 1: passes at once for j = 0) after it has
+//                              issued every k-block of tile j, so the ring never waits for an epilogue.
+//   ready (1 + 96 arrivals):   the producer (with the residual's TMA bytes, 0 without a residual) and the epilogue warps
+//                              (tile j's bias rows are in shared memory); the consumers wait for it after their main loop.
+//   full  (256 arrivals):      every consumer thread has written its part of tile j (and fenced it for the async proxy);
+//                              the epilogue warps wait for it.  They stage tile j + 1's bias only after it, so the bias
+//                              buffer is single.
+// Each barrier's phase j + 1 can only start after phase j has completed (ready(j + 1) follows full(j), full(j + 1) follows
+// ready(j + 1), free(j + 1) follows full(j + 1)), so one parity bit per barrier is enough.  A ragged last n-tile moves only
+// its n_out - n0 columns (whole sub-tiles); rows outside the tensor are zero-filled on the residual load and clipped on the
+// store by the TMA unit, and the column statistics skip them.  A CTA with no tile runs none of this.
 template <int BN, int MINB, bool GEGLU, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, MINB)
 igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-             const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
-  using CF = Cfg<BN, MINB>;
+             const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+             const __grid_constant__ CUtensorMap tmRes, const IgemmParams p) {
+  using CF = Cfg<BN, MINB, GEGLU>;
   constexpr int STAGES = CF::STAGES;
-  constexpr int OUT_BN = GEGLU ? BN / 2 : BN;
+  constexpr int OUT_BN = CF::OUT_BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smA = smem;
   uint8_t* smB = smA + STAGES * A_STAGE_BYTES;
-  float* sstats = reinterpret_cast<float*>(smB + STAGES * CF::B_STAGE_BYTES);
-  uint8_t* slabs = reinterpret_cast<uint8_t*>(sstats) + CF::STATS_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(slabs + NUM_CONSUMER_WARPS * 2 * SLAB_BYTES);
+  uint8_t* stile = smB + STAGES * CF::B_STAGE_BYTES;
+  float* sbias = reinterpret_cast<float*>(stile + CF::OUT_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + CF::BIAS_FLOATS);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
+  uint64_t* free_bar = bars + 2 * STAGES;
+  uint64_t* ready_bar = free_bar + 1;
+  uint64_t* out_full_bar = free_bar + 2;
 
   const int wg = static_cast<int>(threadIdx.x) >> 7;
   const int warp = static_cast<int>(threadIdx.x) >> 5;
@@ -121,27 +154,38 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
   const int kb_per_tap = p.kb_per_tap;
   const int k_iters = p.num_taps * kb_per_tap;
+  const bool direct = (p.flags & AAB_F_DIRECT) != 0;
+  const bool staged = BN >= 64 && (GEGLU || !direct);
+  const bool has_res = !GEGLU && p.residual != nullptr;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmA2);
     prefetch_tmap(&tmB);
+    if (staged) {
+      prefetch_tmap(&tmOut);
+      if (has_res) prefetch_tmap(&tmRes);
+    }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], NUM_CONSUMER_WARPS);   // lane 0 of every consumer warp releases a stage
+      mbar_init(&empty_bar[i], NUM_CONSUMERS * 4);   // lane 0 of every consumer warp releases a stage
     }
+    mbar_init(free_bar, NUM_EPI_THREADS);
+    mbar_init(ready_bar, 1 + NUM_EPI_THREADS);
+    mbar_init(out_full_bar, NUM_CONSUMER_THREADS);
     fence_barrier_init();
   }
   __syncthreads();
 
   if (wg == 0) {
-    // ===================================================== TMA producer
     setmaxnreg_dec<CF::PRODUCER_REGS>();
-    if (warp == 0 && elect_one()) {
+    if (warp == 0) {
+      // ===================================================== TMA producer
+      if (!elect_one()) return;
       // the weight tile is fetched in NS row slices of BN / NS rows (GEGLU: values and gates are separate slices)
       constexpr int NS = GEGLU ? 2 : 1;
       constexpr int slice_rows = BN / NS;
-      uint32_t it = 0;
+      uint32_t it = 0, j = 0;
       for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
         const int nt = tile % p.num_n_tiles;
         int mt = tile / p.num_n_tiles;
@@ -170,14 +214,131 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               tma_load_5d(smA + s * A_STAGE_BYTES, &tmA2, &full_bar[s], kc - p.Kc1 + o0, cb[0] + o1, cb[1] + o2,
                           cb[2] + o3, cb[3] + o4);
 #pragma unroll
-            for (int j = 0; j < NS; ++j) {
-              const int t0 = j * slice_rows;                        // first tile row of the slice
+            for (int jn = 0; jn < NS; ++jn) {
+              const int t0 = jn * slice_rows;                       // first tile row of the slice
               const int row = (GEGLU && t0 >= BN / 2) ? p.N / 2 + n0 + (t0 - BN / 2) : n0 + t0;
               tma_load_3d(smB + s * CF::B_STAGE_BYTES + t0 * 128, &tmB, &full_bar[s], kg, row, bbatch);
             }
           }
         }
+        if (staged) {
+          // this tile's staging tile, once the previous tile's has been stored, with the residual in it
+          mbar_wait(free_bar, (j & 1) ^ 1);
+          const int nsub = min(OUT_BN, p.n_out - n0) / SUB_COLS;
+          if (has_res) {
+            mbar_arrive_expect_tx(ready_bar, nsub * SUB_BYTES);
+            for (int s = 0; s < nsub; ++s)
+              tma_load_5d(stile + s * SUB_BYTES, &tmRes, ready_bar, n0 + s * SUB_COLS, cb[0], cb[1], cb[2], cb[3]);
+          } else {
+            mbar_arrive(ready_bar);
+          }
+          ++j;
+        }
       }
+      return;
+    }
+    if (!staged) return;
+    // ===================================================== epilogue warps: bias rows in, column statistics, TMA store out
+    const int et = static_cast<int>(threadIdx.x) - 32;
+    const bool stats = !GEGLU && p.colstats != nullptr;
+    uint32_t j = 0;
+    for (int tile = tile_first; tile < num_tiles; tile += tile_step, ++j) {
+      const int nt = tile % p.num_n_tiles;
+      int mt = tile / p.num_n_tiles;
+      const int mt_lin = mt;                                   // linear m-tile index (row of the column-statistics table)
+      int cb[4], lim[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        cb[i] = (mt % p.tiles[i]) * p.box[i];
+        mt /= p.tiles[i];
+        lim[i] = min(p.box[i], p.dimD[i] - cb[i]);             // rows of the tile inside the tensor along dim i
+      }
+      const int n0 = nt * OUT_BN;
+      const int ncols = min(OUT_BN, p.n_out - n0);
+      // this tile's bias (GEGLU: values | gates) and the per-sample bias of its first and last row's sample (host: a tile
+      // spans at most two samples); the consumers have read the previous tile's (full barrier below)
+      if (p.bias != nullptr)
+        for (int c = et; c < ncols; c += NUM_EPI_THREADS) {
+          sbias[c] = __ldg(p.bias + n0 + c);
+          if (GEGLU) sbias[OUT_BN + c] = __ldg(p.bias + p.N / 2 + n0 + c);
+        }
+      if (!GEGLU && p.bias2 != nullptr) {
+        // (the host keeps the output rows of a staged launch below 2^31)
+        const int g_first = ((cb[3] * p.dimD[2] + cb[2]) * p.dimD[1] + cb[1]) * p.dimD[0] + cb[0];
+        const int g_last = ((((cb[3] + lim[3] - 1) * p.dimD[2] + cb[2] + lim[2] - 1) * p.dimD[1] + cb[1] + lim[1] - 1) *
+                            p.dimD[0]) + cb[0] + lim[0] - 1;
+        const float* b0 = p.bias2 + static_cast<long>(g_first / p.rows_per_bias2) * p.ld_bias2 + n0;
+        const float* b1 = p.bias2 + static_cast<long>(g_last / p.rows_per_bias2) * p.ld_bias2 + n0;
+        for (int c = et; c < ncols; c += NUM_EPI_THREADS) {
+          sbias[OUT_BN + c] = __ldg(b0 + c);
+          sbias[2 * OUT_BN + c] = __ldg(b1 + c);
+        }
+      }
+      mbar_arrive(ready_bar);
+      mbar_wait(out_full_bar, j & 1);
+      if (et == 0) {
+        for (int s = 0; s < ncols / SUB_COLS; ++s)
+          tma_store_5d(&tmOut, stile + s * SUB_BYTES, n0 + s * SUB_COLS, cb[0], cb[1], cb[2], cb[3]);
+        tma_store_commit();
+      }
+      if (stats) {
+        // one column per thread, in the float order of the accumulator layout: consumer warp w holds rows 16 w .. 16 w + 15,
+        // its lane-row r (0..7) sums (0 + v[r]) + v[r + 8] over valid rows, the xor-4 / 8 / 16 butterfly combines the lane-rows
+        // as ((p0 + p1) + (p2 + p3)) + ((p4 + p5) + (p6 + p7)), and the 8 warps are added in order
+        uint32_t vmask[4];                                     // bit r & 31 of word r >> 5: tile row r is inside the tensor
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          int r = static_cast<int>(lane_id()) + 32 * k;
+          bool v = true;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            v = v && (r % p.box[i] < lim[i]);
+            r /= p.box[i];
+          }
+          vmask[k] = __ballot_sync(0xffffffffu, v);
+        }
+        for (int c = et; c < ncols; c += NUM_EPI_THREADS) {
+          auto ld = [&](int r) {
+            const uint16_t u = *reinterpret_cast<const uint16_t*>(stile + stage_word_off(r, c >> 1) + 2 * (c & 1));
+            return bf16 ? __uint_as_float(static_cast<uint32_t>(u) << 16) : __half2float(__ushort_as_half(u));
+          };
+          float tot_s = 0.f, tot_q = 0.f;
+#pragma unroll 1
+          for (int w = 0; w < NUM_CONSUMERS * 4; ++w) {
+            const uint32_t vw = w < 2 ? vmask[0] : w < 4 ? vmask[1] : w < 6 ? vmask[2] : vmask[3];
+            const uint32_t vrows = (w & 1) ? vw >> 16 : vw;    // rows 16 w .. 16 w + 15
+            float ts[4], tq[4];                                // (p0 + p1), (p2 + p3), (p4 + p5), (p6 + p7)
+#pragma unroll
+            for (int r = 0; r < 8; r += 2) {
+              float s2[2], q2[2];
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                float s = 0.f, q = 0.f;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int row = 16 * w + r + u + 8 * h;
+                  if ((vrows >> (r + u + 8 * h)) & 1) {
+                    const float v = ld(row);
+                    s += v;
+                    q = fmaf(v, v, q);
+                  }
+                }
+                s2[u] = s;
+                q2[u] = q;
+              }
+              ts[r / 2] = s2[0] + s2[1];
+              tq[r / 2] = q2[0] + q2[1];
+            }
+            tot_s += (ts[0] + ts[1]) + (ts[2] + ts[3]);
+            tot_q += (tq[0] + tq[1]) + (tq[2] + tq[3]);
+          }
+          float* cs = p.colstats + (static_cast<long>(mt_lin) * p.n_out + n0 + c) * 2;
+          cs[0] = tot_s;
+          cs[1] = tot_q;
+        }
+      }
+      if (et == 0) tma_store_wait_read<0>();
+      mbar_arrive(free_bar);
     }
     return;
   }
@@ -187,11 +348,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int cw = wg - 1;
   const int wq = warp & 3;
   const int lane = static_cast<int>(lane_id());
-  const bool direct = (p.flags & AAB_F_DIRECT) != 0;
   const bool out_f32 = (p.flags & AAB_F_OUT_F32) != 0;
   const bool scale_acc = (p.flags & AAB_F_SCALE_ACC) != 0;
-  const bool stats = !GEGLU && !direct && p.colstats != nullptr;
-  uint32_t it = 0;
+  uint32_t it = 0, j = 0;
 
   for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
     float acc[BN / 2];                  // the first wgmma of a tile overwrites it (scale-d = 0)
@@ -220,7 +379,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // ---------------- epilogue
     const int nt = tile % p.num_n_tiles;
     int mt = tile / p.num_n_tiles;
-    const int mt_lin = mt;                                  // linear m-tile index (row of the column-statistics table)
     int cb[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -245,83 +403,50 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       grow[h] = ((static_cast<long>(g[3]) * p.dimD[2] + g[2]) * p.dimD[1] + g[1]) * p.dimD[0] + g[0];
     }
     const int n0 = nt * OUT_BN;
-    // per-sample bias row and residual row of a valid accumulator row (formed where used: pointers kept across the
-    // epilogue would not fit beside a 256-column accumulator)
-    auto bias2row = [&](int h) { return p.bias2 + (grow[h] / p.rows_per_bias2) * p.ld_bias2; };
-    auto resrow = [&](int h) { return reinterpret_cast<const uint8_t*>(p.residual) + grow[h] * p.ld_res * 2; };
     const bool has_bias2 = p.bias2 != nullptr;
-    if (stats) named_bar_sync(1, 128 * NUM_CONSUMERS);     // the previous tile's statistics scratch has been read
 
     if (GEGLU || !direct) {
       if constexpr (BN >= 64) {
-        // ---- staged: the warp converts 32 columns of its 16 rows at a time into its slab, then the slab leaves as 16-byte
-        // pieces of whole 64-byte row segments.  In both views of the slab a thread owns rows (lane >> 2) and (lane >> 2) + 8:
-        // as words of chunk j (accumulator layout, columns 8 j + 2 (lane & 3)) and as the whole chunk (lane & 3).  The
-        // residual takes the same way in.  Global stores are not waited for: the warp is back in the main loop of its next
-        // tile while they drain.
+        // ---- staged: bias, per-sample bias, residual, activation and rounding in the accumulator layout, written in place
+        // over the residual in the staging tile; the warps 1 - 3 of warpgroup 0 take it from there
         const int q = lane & 3;
-        const int sw = (lane >> 3) & 3;                        // chunk swizzle of both rows (row pair index mod 4)
-        uint8_t* const srow0 = slabs + (cw * 4 + wq) * 2 * SLAB_BYTES + (lane >> 2) * (SLAB_COLS * 2);
-        constexpr int H_OFF = 8 * SLAB_COLS * 2;               // row r + 8 of the slab
-        const int vec_off = (q ^ sw) << 4;
-        const int nslab = (min(OUT_BN, p.n_out - n0)) / SLAB_COLS;   // n_out is a multiple of 32
-        const bool has_res = !GEGLU && p.residual != nullptr;
-        auto fetch_res = [&](int s) {                          // residual of slab s -> slab buffer s & 1, no registers held
+        const int r0 = cw * 64 + wq * 16 + (lane >> 2);        // tile rows r0 and r0 + 8
+        const int nslab = min(OUT_BN, p.n_out - n0) / SUB_COLS;   // n_out is a multiple of 32
+        int bsel[2] = {0, 0};                                  // per-sample bias row of each accumulator row (0: first sample)
+        if (!GEGLU && has_bias2) {
+          const long s_first =
+              (((static_cast<long>(cb[3]) * p.dimD[2] + cb[2]) * p.dimD[1] + cb[1]) * p.dimD[0] + cb[0]) / p.rows_per_bias2;
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-            if (rvalid[h])
-              cp_async_16(srow0 + (s & 1) * SLAB_BYTES + h * H_OFF + vec_off, resrow(h) + (n0 + s * SLAB_COLS + 8 * q) * 2);
-          cp_async_commit();
-        };
-        // bias of slab s (GEGLU: value and gate columns) in registers one slab ahead: a load issued where it is added would
-        // put an L2 round trip on the conversion path of every slab
-        float2 bval[2][SLAB_COLS / 8], bgate[2][SLAB_COLS / 8];
-        auto fetch_bias = [&](int s) {
+          for (int h = 0; h < 2; ++h) bsel[h] = (grow[h] / p.rows_per_bias2 > s_first) ? 2 * OUT_BN : OUT_BN;
+        }
+        mbar_wait(ready_bar, j & 1);
 #pragma unroll
-          for (int j = 0; j < SLAB_COLS / 8; ++j) {
-            const int col = n0 + s * SLAB_COLS + j * 8 + 2 * q;
-            bval[s & 1][j] = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-            if (GEGLU) bgate[s & 1][j] = __ldg(reinterpret_cast<const float2*>(p.bias + p.N / 2 + col));
-          }
-        };
-        if (p.bias != nullptr && nslab > 0) fetch_bias(0);
-        __syncwarp();                                          // the previous tile's last slab has been read
-        if (has_res) fetch_res(0);
-#pragma unroll
-        for (int s = 0; s < OUT_BN / SLAB_COLS; ++s) {
+        for (int s = 0; s < OUT_BN / SUB_COLS; ++s) {
           if (s >= nslab) break;                               // warp-uniform: a ragged last n-tile
-          uint8_t* const sb = srow0 + (s & 1) * SLAB_BYTES;
-          if (has_res) cp_async_wait<0>();
-          __syncwarp();                                        // this slab's residual has landed; the other buffer has been read
-          if (has_res && s + 1 < nslab) fetch_res(s + 1);      // in flight while this slab is converted
-          if (p.bias != nullptr && s + 1 < nslab) fetch_bias(s + 1);
 #pragma unroll
-          for (int j = 0; j < SLAB_COLS / 8; ++j) {
-            const int jj = s * (SLAB_COLS / 8) + j;
+          for (int jc = 0; jc < SUB_COLS / 8; ++jc) {
+            const int jj = s * (SUB_COLS / 8) + jc;
             const int cl = jj * 8 + 2 * q;                     // tile column of this thread's pair
-            const int col = n0 + cl;
-            const int word_off = ((j ^ sw) << 4) + q * 4;
-            float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               float x[2] = {acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]};
-              uint32_t* wp = reinterpret_cast<uint32_t*>(sb + h * H_OFF + word_off);
+              uint32_t* wp = reinterpret_cast<uint32_t*>(stile + stage_word_off(r0 + 8 * h, cl >> 1));
               if (GEGLU) {
                 float g[2] = {acc[4 * (jj + BN / 16) + 2 * h], acc[4 * (jj + BN / 16) + 2 * h + 1]};
                 if (p.bias != nullptr) {
-                  const float2 bv = bval[s & 1][j];
-                  const float2 bg = bgate[s & 1][j];
+                  const float2 bv = *reinterpret_cast<const float2*>(sbias + cl);
+                  const float2 bg = *reinterpret_cast<const float2*>(sbias + OUT_BN + cl);
                   x[0] += bv.x; x[1] += bv.y;
                   g[0] += bg.x; g[1] += bg.y;
                 }
                 *wp = pack2(x[0] * gelu_fast_f(g[0]), x[1] * gelu_fast_f(g[1]), bf16);
               } else {
                 if (p.bias != nullptr) {
-                  const float2 b = bval[s & 1][j];
+                  const float2 b = *reinterpret_cast<const float2*>(sbias + cl);
                   x[0] += b.x; x[1] += b.y;
                 }
                 if (has_bias2 && rvalid[h]) {
-                  const float2 b = __ldg(reinterpret_cast<const float2*>(bias2row(h) + col));
+                  const float2 b = *reinterpret_cast<const float2*>(sbias + bsel[h] + cl);
                   x[0] += b.x; x[1] += b.y;
                 }
                 if (has_res) {
@@ -332,42 +457,18 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                   x[0] = silu_fast_f(x[0]);
                   x[1] = silu_fast_f(x[1]);
                 }
-                const uint32_t o = pack2(x[0], x[1], bf16);
-                *wp = o;
-                if (stats && rvalid[h]) {
-                  const float2 f = unpack2(o, bf16);           // statistics of the ROUNDED 16-bit outputs
-                  ssum[0] += f.x; ssq[0] = fmaf(f.x, f.x, ssq[0]);
-                  ssum[1] += f.y; ssq[1] = fmaf(f.y, f.y, ssq[1]);
-                }
+                *wp = pack2(x[0], x[1], bf16);
               }
             }
-            if (stats) {
-              // sum over the warp's 16 rows: the 8 lanes sharing (lane & 3) hold this column pair; fixed-order butterfly
-#pragma unroll
-              for (int off = 4; off < 32; off <<= 1) {
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  ssum[e] += __shfl_xor_sync(0xffffffffu, ssum[e], off);
-                  ssq[e] += __shfl_xor_sync(0xffffffffu, ssq[e], off);
-                }
-              }
-              if (lane < 4) {
-                float* sp = sstats + ((cw * 4 + wq) * BN + cl) * 2;
-                sp[0] = ssum[0]; sp[1] = ssq[0]; sp[2] = ssum[1]; sp[3] = ssq[1];
-              }
-            }
-          }
-          __syncwarp();
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (rvalid[h])
-              *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) +
-                                        (grow[h] * p.ld_out + n0 + s * SLAB_COLS + 8 * q) * 2) =
-                  *reinterpret_cast<const uint4*>(sb + h * H_OFF + vec_off);
           }
         }
+        fence_proxy_async_smem();                              // the TMA store reads what this thread wrote
+        mbar_arrive(out_full_bar);
+        ++j;
       }
     } else if constexpr (!GEGLU) {
+      auto bias2row = [&](int h) { return p.bias2 + (grow[h] / p.rows_per_bias2) * p.ld_bias2; };
+      auto resrow = [&](int h) { return reinterpret_cast<const uint8_t*>(p.residual) + grow[h] * p.ld_res * 2; };
       // ---- direct: masked per element, straight from the accumulator registers
 #pragma unroll
       for (int jj = 0; jj < OUT_BN / 8; ++jj) {
@@ -394,21 +495,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             }
           }
         }
-      }
-    }
-    if (stats) {
-      // the eight warps' partial sums, added in warp order -> one (sum, sumsq) pair per column and m-tile, reproducible
-      named_bar_sync(1, 128 * NUM_CONSUMERS);
-      for (int c = static_cast<int>(threadIdx.x) - 128; c < OUT_BN; c += 128 * NUM_CONSUMERS) {
-        if (n0 + c >= p.n_out) break;
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int w = 0; w < NUM_CONSUMER_WARPS; ++w) {
-          s0 += sstats[(w * BN + c) * 2];
-          s1 += sstats[(w * BN + c) * 2 + 1];
-        }
-        p.colstats[(static_cast<long>(mt_lin) * p.n_out + n0 + c) * 2] = s0;
-        p.colstats[(static_cast<long>(mt_lin) * p.n_out + n0 + c) * 2 + 1] = s1;
       }
     }
   }
@@ -468,23 +554,23 @@ int num_sms() {
 }
 
 template <int BN, int MINB, bool GEGLU, bool BF16>
-static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
-                    cudaStream_t stream) {
-  using CF = Cfg<BN, MINB>;
+static int launch_t(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const CUtensorMap& o,
+                    const CUtensorMap& r, const IgemmParams& p, cudaStream_t stream) {
+  using CF = Cfg<BN, MINB, GEGLU>;
   static std::atomic<unsigned long long> attr_done{0};
   if (int r = ensure_dyn_smem(igemm_kernel<BN, MINB, GEGLU, BF16>, CF::SMEM_BYTES, attr_done)) return r;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   int ctas = num_sms() * MINB;     // persistent: MINB CTAs per SM
   if (tiles < ctas) ctas = tiles;
-  igemm_kernel<BN, MINB, GEGLU, BF16><<<ctas, NUM_THREADS, CF::SMEM_BYTES, stream>>>(a, a2, b, p);
+  igemm_kernel<BN, MINB, GEGLU, BF16><<<ctas, NUM_THREADS, CF::SMEM_BYTES, stream>>>(a, a2, b, o, r, p);
   return cudaGetLastError() == cudaSuccess ? AAB_OK : AAB_ERR_CUDA;
 }
 
 template <int BN, bool GEGLU, int MINB = 1>
-static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const IgemmParams& p,
-                     cudaStream_t stream) {
-  if (p.flags & AAB_F_BF16) return launch_t<BN, MINB, GEGLU, true>(a, a2, b, p, stream);
-  return launch_t<BN, MINB, GEGLU, false>(a, a2, b, p, stream);
+static int launch_bn(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b, const CUtensorMap& o,
+                     const CUtensorMap& r, const IgemmParams& p, cudaStream_t stream) {
+  if (p.flags & AAB_F_BF16) return launch_t<BN, MINB, GEGLU, true>(a, a2, b, o, r, p, stream);
+  return launch_t<BN, MINB, GEGLU, false>(a, a2, b, o, r, p, stream);
 }
 
 }  // namespace aab
@@ -497,8 +583,22 @@ static int igemm_is_staged(const AabIgemmDesc* d) {
   const int bn = d->block_n;
   const int n_out = geglu ? d->n / 2 : d->n;
   if ((d->flags & (AAB_F_DIRECT | AAB_F_OUT_F32 | AAB_F_SCALE_ACC)) || bn == 32 || (d->ld_out % 8) || (n_out % 32)) return 0;
-  if (reinterpret_cast<uintptr_t>(d->out) % 16) return 0;   // rows are stored and the residual is read 16 bytes at a time
-  if (d->residual && ((d->ld_res % 8) || reinterpret_cast<uintptr_t>(d->residual) % 16)) return 0;
+  // the output (and the residual) move as TMA boxes of a 5-D map [pixel dims][n_out]: 16-byte aligned base, row strides a
+  // multiple of 16 bytes, every stride below 2^40 bytes; fewer than 2^31 rows (32-bit row arithmetic in the epilogue warps)
+  long rows = 1;
+  for (int i = 0; i < 4; ++i) rows *= d->dim_d[i] > 0 ? d->dim_d[i] : 1;
+  if (rows >= (1l << 31) || reinterpret_cast<uintptr_t>(d->out) % 16 || rows * d->ld_out * 2 >= (1l << 40)) return 0;
+  if (d->residual && ((d->ld_res % 8) || reinterpret_cast<uintptr_t>(d->residual) % 16 || rows * d->ld_res * 2 >= (1l << 40)))
+    return 0;
+  if (d->bias2) {
+    // the epilogue holds the per-sample bias of two samples per tile: the rows a tile can span must fit in one sample
+    long span = 1, pitch = 1;
+    for (int i = 0; i < 4; ++i) {
+      span += static_cast<long>(d->box[i] - 1) * pitch;
+      pitch *= d->dim_d[i];
+    }
+    if (span > (d->rows_per_bias2 > 0 ? d->rows_per_bias2 : 1)) return 0;
+  }
   if ((d->act == AAB_ACT_GELU || d->act == AAB_ACT_QUICK_GELU) && !geglu) return 0;
   const int extras = (d->residual ? 1 : 0) + (d->bias2 ? 1 : 0) + (d->act == AAB_ACT_SILU ? 1 : 0);
   if (!geglu && (extras > 1 || d->out_scale != 1.0f)) return 0;
@@ -518,7 +618,7 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
   int bn = d->block_n;
   if (bn != 32 && bn != 64 && bn != 128 && bn != 160 && bn != 192 && bn != 256) return AAB_ERR_ARG;
   const int n_out = geglu ? d->n / 2 : d->n;
-  // staged: one extra term (residual | per-sample bias | SiLU), no output scaling, 16-bit rows that can move 16 bytes at a time
+  // staged: one extra term (residual | per-sample bias | SiLU), no output scaling, output and residual addressable by TMA
   const bool direct = !igemm_is_staged(d);
   if (geglu) {   // the gate half of the tile must be a whole number of 64-column blocks; GEGLU only has the staged epilogue
     if ((bn != 128 && bn != 256) || direct || d->residual || d->bias2 || d->act == AAB_ACT_SILU || d->out_scale != 1.0f)
@@ -586,18 +686,33 @@ extern "C" int aab_igemm(const AabIgemmDesc* d, void* stream_) {
     int r = make_tmap_16(&tmB, d->b, 3, dims, strides, box, is_bf16, 128);
     if (r) return r;
   }
-  if (two_cta) return launch_bn<64, false, 2>(tmA, tmA2, tmB, p, stream);
+  CUtensorMap tmOut = tmA, tmRes = tmA;   // staged epilogue only: the output tile leaves and the residual comes in by TMA
+  if (!direct) {
+    long dims[5] = {n_out, d->dim_d[0], d->dim_d[1], d->dim_d[2], d->dim_d[3]};
+    long strides[5] = {1, d->ld_out, 0, 0, 0};
+    for (int i = 2; i < 5; ++i) strides[i] = strides[i - 1] * dims[i - 1];
+    int box[5] = {SUB_COLS, d->box[0], d->box[1], d->box[2], d->box[3]};
+    int r = make_tmap_16(&tmOut, d->out, 5, dims, strides, box, is_bf16, 64);
+    if (r) return r;
+    if (d->residual && !geglu) {
+      strides[1] = d->ld_res;
+      for (int i = 2; i < 5; ++i) strides[i] = strides[i - 1] * dims[i - 1];
+      r = make_tmap_16(&tmRes, d->residual, 5, dims, strides, box, is_bf16, 64);
+      if (r) return r;
+    }
+  }
+  if (two_cta) return launch_bn<64, false, 2>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
   if (geglu) {
-    if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, p, stream);
-    return launch_bn<256, true>(tmA, tmA2, tmB, p, stream);
+    if (bn == 128) return launch_bn<128, true>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    return launch_bn<256, true>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
   }
   switch (bn) {
-    case 32: return launch_bn<32, false>(tmA, tmA2, tmB, p, stream);
-    case 64: return launch_bn<64, false>(tmA, tmA2, tmB, p, stream);
-    case 128: return launch_bn<128, false>(tmA, tmA2, tmB, p, stream);
-    case 160: return launch_bn<160, false>(tmA, tmA2, tmB, p, stream);
-    case 192: return launch_bn<192, false>(tmA, tmA2, tmB, p, stream);
-    default: return launch_bn<256, false>(tmA, tmA2, tmB, p, stream);
+    case 32: return launch_bn<32, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    case 64: return launch_bn<64, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    case 128: return launch_bn<128, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    case 160: return launch_bn<160, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    case 192: return launch_bn<192, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
+    default: return launch_bn<256, false>(tmA, tmA2, tmB, tmOut, tmRes, p, stream);
   }
 }
 
